@@ -6,16 +6,16 @@
 
 Workload (BASELINE.json configs[1]): EDM CIFAR-10 32x32 DDPM++ U-Net (random init, de-zeroed so |F_x| = O(1)), Heun sampler,
 num_steps=10 => NFE=18, batch 512 per GPU, synthetic Gaussian latents.  One "step" = one full sampling pass over one batch.
-`value` = images/sec with latents resident in HBM; `e2e` = the same through the public API with pinned-host latents copied in
-and finished images copied back every step.  Scaling is weak: every rank samples its own 512-image batch, no collective on
+`value` = images/sec with latents resident in HBM.  Scaling is weak: every rank samples its own 512-image batch, no collective on
 the sampling path; one NCCL all_gather of the uint8 images after the timed region (what FID consumes).
 
-At N=1 the same line also carries (rank 0, after the headline measurement; `--no_extras` skips them):
+By default the line carries the headline measurement only, so a run costs about (warmup + steps) sampling passes plus the net build.
+`--extras` adds (rank 0, after the headline measurement) `e2e` (the same through the public API with pinned-host latents copied in and
+finished images copied back every step), the roofline / fp16 legs, and at N=1:
   `configs`    BASELINE configs 3, 4 and 5 (FFHQ-64 iPNDM NFE=6, ImageNet-64 DPM-Solver++(2M) NFE=10, SD-v1.5 AMED-DPM++ NFE=5) measured the
-               same way (value, e2e, roofline, precision) at their per-GPU batch, >= 10 timed steps each;
+               same way (value, e2e, roofline, precision) at their per-GPU batch, `--config_steps` timed steps each;
   `gpu_eager`  the reference's own GPU path -- eager PyTorch (cuDNN / cuBLAS: F.conv2d, F.group_norm, einsum attention), stated through the
-               functional nets of oracle/ (bit-identical to the reference modules on CPU, tests/golden) -- on the same B200, same batch / NFE:
-               the "beat PyTorch-eager on the same GPU" bar of SURVEY.md section 2.2.  A comparator, never the thing measured as `value`.
+               functional nets of oracle/ (bit-identical to the reference modules on CPU, tests/golden) -- on the same GPU, same batch / NFE.  A comparator, never the thing measured as `value`.
 """
 import argparse
 import json
@@ -49,13 +49,20 @@ def parse():
                          "pass; auto (default): the fastest mode whose final images stay within the 1e-3 contract for the named net (PRECISION_FOR)")
     ap.add_argument('--f8_min_channels', type=int, default=0, help='fp16f8 only: blocks with fewer input or output channels stay fp16x3 (0 = all blocks in f8)')
     ap.add_argument('--cpu_batch', type=int, default=8, help='batch of the bounded CPU-baseline sample')
-    ap.add_argument('--no_cpu_baseline', action='store_true')
+    ap.add_argument('--cpu_baseline', action='store_true', help='also time the bounded CPU-baseline sample (N=1)')
     ap.add_argument('--fuse_stats', type=int, default=1, help='1 (default): GroupNorm statistics from the GEMM epilogues; 0: separate gn_stats pass')
-    ap.add_argument('--no_extras', action='store_true', help='skip the roofline / e2e / fp16 legs (timing of the main leg is unchanged)')
-    ap.add_argument('--all_configs', type=int, default=1, help='1 (default, N=1 only): also measure BASELINE configs 3-5 into `configs`')
-    ap.add_argument('--config_steps', type=int, default=10, help='timed steps of each `configs` entry')
-    ap.add_argument('--gpu_eager', type=int, default=1, help='1 (default, N=1 only): time the eager-PyTorch GPU path of the same configs')
+    ap.add_argument('--extras', action='store_true', help='also run the e2e / roofline / fp16 legs and, at N=1, the options below '
+                                                             '(timing of the main leg is unchanged)')
+    ap.add_argument('--all_configs', type=int, default=1, help='1 (default, N=1 with --extras): also measure BASELINE configs 3-5 into `configs`')
+    ap.add_argument('--config_steps', type=int, default=None, help='timed steps of each `configs` entry (default: --steps)')
+    ap.add_argument('--gpu_eager', type=int, default=1, help='1 (default, N=1 with --extras): time the eager-PyTorch GPU path of the same configs')
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='write the images of the last timed step to DIR/<name>.npy (float32; rank 0) for output-by-output comparison of builds')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be >= 1')
+    if args.config_steps is None:
+        args.config_steps = args.steps
     args.precision_requested = args.precision
     args.f8_min_channels_requested = args.f8_min_channels
     if args.precision == 'auto':
@@ -72,11 +79,11 @@ def peaks():
             d = json.load(f)
         return dict(hbm_gbs=d['hbm_gbs'], tflops_burst=d['bf16_tflops'], tflops_sustained=d.get('bf16_tflops_sustained', d['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source='H100 SXM data sheet (700 W; not measured)')
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region (read-only queries)."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
 
@@ -124,14 +131,13 @@ class ClockSampler:
 # ---------------------------------------------------------------------------------------------------------------------
 def cpu_reference_leg(args, steps, warmup):
     """The reference's CPU path on the host cores: the oracle port of solvers.<solver>_sampler on EDMPrecond (oracle/ is pinned
-    bit-exact to /root/reference by tests/golden; /root/reference itself does not exist on the GPU box).  Bounded sample:
+    bit-exact to the reference by tests/golden).  Bounded sample:
     the same net / solver / NFE on a batch of `cpu_batch` images."""
     import torch
     from oracle import edm_oracle as O
     from oracle import solvers_oracle as SO
-    # thread count: measured on the B200 host (profiles/cpu_thread_sweep.py, 128 logical CPUs): one CIFAR-net forward at batch 8
-    # takes 0.21 s with 16 threads, 0.27 s with 32, 0.59 s with 64 and 4.6 s with 128 (oversubscription), so the baseline uses
-    # the fastest setting rather than every logical CPU.
+    # thread count: at batch 8 the CIFAR-net forward does not scale past ~16 threads and slows down sharply when every logical CPU of
+    # a large host is used (oversubscription), so the baseline caps the count (DSB_CPU_THREADS overrides).
     cores = min(os.cpu_count() or 1, int(os.environ.get('DSB_CPU_THREADS', '16')))
     torch.set_num_threads(cores)
     P, S = O.make_net(args.net, seed=0, dezero=True)
@@ -158,7 +164,7 @@ def make_config(args, world):
     return dict(workload=f'EDM {args.net} U-Net, {args.solver} num_steps={args.num_steps} (NFE={nfe}), batch {args.batch}/GPU',
                 net=args.net, solver=args.solver, nfe=nfe, batch_per_gpu=args.batch, global_batch=args.batch * max(world, 1),
                 weights='random init (reference constructors, seed 0), init_zero layers de-zeroed', parallelism=f'dp{world}',
-                l2='per-forward activation working set (GBs) >> 126 MB L2')
+                l2='per-forward activation working set (GBs) >> 50 MB L2')
 
 
 def build_workload(args, dev, rank):
@@ -289,10 +295,12 @@ def main():
     launches = net.total_launches + solver_utils.LAUNCHES[0] - l0
     clk = clocks.stop() if rank == 0 else None
     value = world * B * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(images=images))
 
     # ---- end-to-end through the public API with host buffers -------------------------------------------------------
     e2e = None
-    if not args.no_extras:
+    if args.extras:
         e2e = measure_e2e(sampler, net, kw, shape, args.steps, barrier, dev, world)
 
     # ---- finished samples: FID statistics path over NCCL (outside the timed region) ------------------------------------
@@ -354,12 +362,12 @@ def main():
         line['gits_nccl'] = gits_nccl
 
     try:
-        if not args.no_extras:
+        if args.extras:
             extras(args, line, net, sampler, kw, latents, labels, images, B, dev, pk)
     except Exception as e:                       # the main measurement above is already complete; report instead of dying
         line['extras_error'] = repr(e)
 
-    solo = world == 1 and not args.no_extras
+    solo = world == 1 and args.extras
     if solo and args.gpu_eager and args.net != 'sd15':
         try:
             line['gpu_eager'] = gpu_eager_leg(args, dev, native_value=value)
@@ -370,7 +378,7 @@ def main():
         torch.cuda.empty_cache()
         line['configs'] = other_configs(args, dev, pk)
 
-    if not args.no_cpu_baseline and world == 1:
+    if args.cpu_baseline and world == 1:
         cb = cpu_reference_leg(args, 1, 1)
         line['cpu_baseline'] = dict(value=cb['value'], unit='images/s', cores=cb['cores'], kind='port', sample=cb['sample'])
     print(json.dumps(line), flush=True)
@@ -379,17 +387,31 @@ def main():
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, arrays, limit_bytes=64 << 20):
+    """arrays -> out_dir/<name>.npy as float32.  An array above the byte budget keeps a fixed, seeded subset of its leading (batch) index,
+    so two runs with the same arguments write the same elements."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    budget = limit_bytes // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > budget:
+            keep = max(1, budget // (a[0].nbytes or 1))
+            a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def DTYPE_TEXT(precision):
-    return 'fp16 operands, fp32 accumulate' + {'fp16x3': ' (split-precision: 3 tcgen05 MMAs per product)',
+    return 'fp16 operands, fp32 accumulate' + {'fp16x3': ' (split-precision: 3 wgmma MMAs per product)',
                                                'fp16f8': ' (split-precision: fp16 hi x hi + two e4m3 correction MMAs per product)'}.get(precision, '')
 
 
 # BASELINE.json configs[2..4] at their per-GPU batch (1024 / 4, 2048 / 8, 64 / 8 images per GPU)
 OTHER_CONFIGS = [
-    dict(id=3, net='ffhq', solver='ipndm', num_steps=7, batch=256, baseline='EDM FFHQ-64, iPNDM NFE=6 (4-term multistep history), batch 1024 on 4xB200'),
+    dict(id=3, net='ffhq', solver='ipndm', num_steps=7, batch=256, baseline='EDM FFHQ-64, iPNDM NFE=6 (4-term multistep history), batch 1024 on 4 GPUs'),
     dict(id=4, net='imagenet64', solver='dpm_pp', num_steps=11, batch=256,
-         baseline='EDM ImageNet-64 class-cond, DPM-Solver++(2M) NFE=10 with GITS schedule, batch 2048 on 8xB200'),
-    dict(id=5, net='sd15', solver='amed_dpm_pp', num_steps=4, batch=8, baseline='Stable Diffusion v1.5 latent 512x512, AMED-plugin on DPM++ NFE=5, batch 64 on 8xB200'),
+         baseline='EDM ImageNet-64 class-cond, DPM-Solver++(2M) NFE=10 with GITS schedule, batch 2048 on 8 GPUs'),
+    dict(id=5, net='sd15', solver='amed_dpm_pp', num_steps=4, batch=8, baseline='Stable Diffusion v1.5 latent 512x512, AMED-plugin on DPM++ NFE=5, batch 64 on 8 GPUs'),
 ]
 
 
@@ -457,7 +479,7 @@ def other_configs(args, dev, pk):
 
 
 def gpu_eager_leg(args, dev, native_value, t_steps=None, solver_kw=None):
-    """The reference's GPU path on this B200: eager PyTorch (cuDNN convolutions, cuBLAS einsum attention, ATen elementwise solver steps)
+    """The reference's GPU path on this GPU: eager PyTorch (cuDNN convolutions, cuBLAS einsum attention, ATen elementwise solver steps)
     through oracle/'s functional restatement of the reference modules (networks_edm.py:60-82 conv2d path, :96-98 group_norm, :105-118
     attention; solvers.py loops), same net / batch / NFE / latents shape.  Three settings:
       default  torch defaults, which is what sample.py runs with: cuDNN TF32 convolutions on, fp32 matmuls (sample.py sets no flags)
@@ -612,29 +634,16 @@ def sd15_param_shapes():
 
 
 # `--precision auto`: the fastest precision whose FINAL IMAGES hold max-abs <= 1e-3 against the reference on that net's BASELINE config
-# (de-zeroed random-init weights).  Measured on B200 (profiles/r01d, tests/test_gpu_parity.py::test_fullsize_sampler_parity_f8_mode):
-#   cifar10  Heun NFE=18      fp16f8 vs fp16x3 2.7e-4 (+ fp16x3 vs reference <= 1.5e-4)            -> fp16f8
-#   imagenet64 DPM++ NFE=10   3.5e-5                                                             -> fp16f8
-#   ffhq     iPNDM NFE=6      all blocks in f8: 1.08e-3, over the gate (this net amplifies GEMM rounding the most); f8 only in the blocks
-#                             with >= 256 channels (F8_MIN_CHANNELS_FOR): 6.2e-4 at batch 256 (profiles/r02b)     -> fp16f8, f8_min_channels 256
-#   sd15     AMED-DPM++ NFE=5  fp16f8 (+ f8_linear) vs fp16x3: 1.4e-2 on latents of magnitude 80 = 1.8e-4 relative (profiles/r02c; the
-#                             latent-diffusion tests hold 1e-3 x max|x|, the scale of the random-weight net's latents)      -> fp16f8
+# (de-zeroed random-init weights); held by tests/test_gpu_parity.py (the f8-mode parity tests).  FFHQ amplifies GEMM rounding the most:
+# with every block in f8 it misses the gate, so there f8 runs only in the blocks with >= 256 channels (F8_MIN_CHANNELS_FOR).
 PRECISION_FOR = {'cifar10': 'fp16f8', 'imagenet64': 'fp16f8', 'ffhq': 'fp16f8', 'sd15': 'fp16f8'}
 # with fp16f8: blocks narrower than this stay fp16x3 (plan.pack_weights).  Only nets whose all-f8 run misses the gate need it.
 F8_MIN_CHANNELS_FOR = {'ffhq': 256}
 
 
-# DRAM bytes (dram__bytes_read.sum + dram__bytes_write.sum) of ONE launch of the named GEMM, from `ncu --set full` captures of this
-# bench command committed under profiles/ (a number measured under the profiler is a byte count, not a time).
-NCU_TRAFFIC = {
-    ('conv3x3 256->256 @32x32 x512', 'fp16x3'): (0.539457e9 + 0.496578e9, 'profiles/r01b_ncu_gemm_conv_b512.txt (launch id 1)'),
-    ('conv3x3 256->256 @32x32 x512 f8', 'fp16f8'): (0.540013e9 + 0.496059e9, 'profiles/r02/ncu_gemm_pair_cifar_f8_r02p.txt (gemm_tc_pair_kernel, ncu --set full)'),
-}
-
-
 def dominant_launch(args, line, net):
     """Per-launch view of the GEMM shape that takes the largest share of the forward: algorithmic FLOPs and bytes of one launch
-    (gemm_desc.describe) over its mean CUDA-event time in this run, plus the ncu DRAM traffic of the same launch where a capture exists."""
+    (gemm_desc.describe) over its mean CUDA-event time in this run."""
     from diff_sampler_b200 import _cstructs as S
     from diff_sampler_b200 import gemm_desc as G
     ms, pl = net.last_profile
@@ -648,23 +657,15 @@ def dominant_launch(args, line, net):
         g['n'] += 1
         g['ms'] += ms[i]
     label, g = max(groups.items(), key=lambda kv: kv[1]['ms'])
-    for (lab, prec), _ in NCU_TRAFFIC.items():            # prefer the shape the committed ncu capture shows, when this plan has it
-        if prec == args.precision and lab in groups and groups[lab]['ms'] >= 0.5 * g['ms']:
-            label, g = lab, groups[lab]
     per = g['ms'] / g['n']
-    traffic = NCU_TRAFFIC.get((label, args.precision))
     rl = line['roofline']
     rl['dominant_launch'] = dict(label=label, launches_per_forward=g['n'], ms_per_launch=per, share_of_gemm_time=g['ms'] / rl['gemm_ms_per_forward'],
                                  algorithmic_flops=g['flops'], achieved_tflops=g['flops'] / (per / 1e3) / 1e12,
-                                 frac_of_peak=g['flops'] / (per / 1e3) / 1e12 / rl['peak'], algorithmic_bytes=g['bytes'],
-                                 traffic=traffic[0] if traffic else None, traffic_source=traffic[1] if traffic else None)
-    if traffic:
-        rl['traffic'] = traffic[0]
-        rl['traffic_note'] = f'per launch of the dominant GEMM ({label}): algorithmic {g["bytes"] / 1e9:.3f} GB; ' + traffic[1]
+                                 frac_of_peak=g['flops'] / (per / 1e3) / 1e12 / rl['peak'], algorithmic_bytes=g['bytes'])
 
 
 def roofline_leg(args, line, net, latents, labels, B, dev, pk, kw):
-    """Roofline of the dominant kernel (the tcgen05 GEMM / conv kernel), measured live: every op of one denoiser evaluation is bracketed by
+    """Roofline of the dominant kernel (the wgmma GEMM / conv kernel), measured live: every op of one denoiser evaluation is bracketed by
     CUDA events on the launch stream (ds_unet_set_profiling); achieved = algorithmic FLOPs of one evaluation / summed GEMM time."""
     import torch
     from diff_sampler_b200 import _cstructs as S
@@ -695,7 +696,7 @@ def roofline_leg(args, line, net, latents, labels, B, dev, pk, kw):
     f1.record()
     torch.cuda.synchronize()
     line['roofline'] = dict(bound='tensor', achieved=achieved, peak=peak, unit='TFLOP/s', frac=(achieved / peak) if achieved else None,
-                            traffic=None, kernel='gemm_tc_pair_kernel / gemm_tc_kernel (+ attn3_kernel): all conv / linear / attention contractions of one denoiser evaluation',
+                            traffic=None, kernel='gemm_tc_kernel (+ attn_kernel): all conv / linear / attention contractions of one denoiser evaluation',
                             algorithmic_flops_per_forward=flops, launches_per_forward=gemm_n + attn_n, gemm_ms_per_forward=gemm_ms,
                             attn_ms_per_forward=attn_ms, all_ops_ms_per_forward=fwd_ms, forward_ms_back_to_back=f0.elapsed_time(f1) / n_rep,
                             gemm_share_of_forward=tc_ms / fwd_ms if fwd_ms else None,
@@ -741,7 +742,7 @@ def extras(args, line, net, sampler, kw, latents, labels, images, B, dev, pk):
                                        kernel='update_kernel<0, EPS> (Euler step: read x, D; write x+)', bytes_per_launch=3 * n * 4,
                                        peak_source=pk['source'])
         # the same kernel at the BASELINE shape (Heun corrector on [B,3,32,32]: read x, x_pred, D', d; write x+ = 20 B/elem): these
-        # 6 MB tensors live in the 126 MB L2, so this is an effective (L2-assisted) bandwidth, reported beside the HBM-resident number
+        # 6 MB tensors live in the 50 MB L2, so this is an effective (L2-assisted) bandwidth, reported beside the HBM-resident number
         xs_ = [torch.randn_like(latents) for _ in range(5)]
         for _ in range(5):
             solver_utils.solver_update(xs_[4], xs_[0], [1.0, 0.1, 0.1], mode=S.DS_M_EPS, D=xs_[1], xs=xs_[2], t=2.0, hist=[xs_[3]])
@@ -771,7 +772,7 @@ def extras(args, line, net, sampler, kw, latents, labels, images, B, dev, pk):
             torch.cuda.synchronize()
             line['fp16_single_pass'] = dict(value=B * args.steps / (f0.elapsed_time(f1) / 1e3), unit='images/s (1 GPU)',
                                             max_abs_vs_fp16x3=(img1 - images).abs().max().item(),
-                                            note='single tcgen05 pass per product; not the headline because it does not hold 1e-3 on the de-zeroed weight set')
+                                            note='single wgmma pass per product; not the headline because it does not hold 1e-3 on the de-zeroed weight set')
             del net1
         # ---- fp16f8 runs: the same sampling pass with the default fp16x3 denoiser, for the speed ratio and the output difference ----
         if args.precision == 'fp16f8':

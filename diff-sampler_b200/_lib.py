@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, 'libdiffsampler_b200.so')
 EXPORTS = [
     'ds_version', 'ds_last_error', 'ds_weights_create', 'ds_weights_destroy', 'ds_unet_create', 'ds_unet_destroy',
     'ds_unet_forward', 'ds_unet_debug_read', 'ds_unet_last_launch_count', 'ds_solver_update', 'ds_dyn_threshold',
-    'ds_op_launch', 'ds_sizeof', 'ds_unet_set_profiling', 'ds_unet_get_profile', 'ds_unet_op_type', 'ds_gits_cost', 'ds_unet_forward_io', 'ds_images_to_uint8', 'ds_solver_update_u8', 'ds_unet_enable_graph', 'ds_amed_predict', 'ds_debug_attn_trace', 'ds_debug_gemm_trace',
+    'ds_op_launch', 'ds_sizeof', 'ds_unet_set_profiling', 'ds_unet_get_profile', 'ds_unet_op_type', 'ds_gits_cost', 'ds_unet_forward_io', 'ds_images_to_uint8', 'ds_solver_update_u8', 'ds_unet_enable_graph', 'ds_amed_predict',
 ]
 
 _lib = None
@@ -52,8 +52,6 @@ def load():
     lib.ds_solver_update_u8.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, C.POINTER(vp), C.c_int, vp, C.c_int, C.c_float, vp,
                                         C.POINTER(C.c_float), vp, C.c_int64, C.c_int, vp]
     lib.ds_amed_predict.argtypes = [vp, C.POINTER(C.c_int), vp, vp, vp, C.c_float, C.c_float, vp, C.c_int, vp]
-    lib.ds_debug_attn_trace.argtypes = [vp, C.c_int]
-    lib.ds_debug_gemm_trace.argtypes = [vp, C.c_int]
     lib.ds_dyn_threshold.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, C.c_float, vp]
     lib.ds_gits_cost.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int64, vp]
     lib.ds_images_to_uint8.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]

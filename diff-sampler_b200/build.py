@@ -1,4 +1,4 @@
-"""Build libdiffsampler_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libdiffsampler_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -7,8 +7,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libdiffsampler_b200.so')
 SOURCES = ['gemm_tc.cu', 'attention.cu', 'elementwise.cu', 'solver.cu', 'engine.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
-              '-Xcompiler', '-fPIC', '--use_fast_math' if False else '-DDSB_NO_FAST_MATH']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
+                     '-Xcompiler', '-fPIC', '--use_fast_math' if False else '-DDSB_NO_FAST_MATH']
 
 
 def _newest_src_mtime():
@@ -24,15 +25,18 @@ def build(force=False, verbose=False):
     if not force and os.path.exists(OUT) and os.path.getmtime(OUT) >= _newest_src_mtime():
         return OUT
     nvcc = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-    objs = []
-    for src in SOURCES:
+    objs, procs = [], []
+    for src in SOURCES:                  # independent translation units: compile them concurrently
         obj = os.path.join(CSRC, src.replace('.cu', '.o'))
         cmd = [nvcc] + NVCC_FLAGS + ['-c', os.path.join(CSRC, src), '-o', obj]
         if verbose:
             print(' '.join(cmd))
-        subprocess.check_call(cmd)
+        procs.append((subprocess.Popen(cmd), cmd))
         objs.append(obj)
-    cmd = [nvcc, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-ldl']
+    for proc, cmd in procs:
+        if proc.wait() != 0:
+            raise subprocess.CalledProcessError(proc.returncode, cmd)
+    cmd = [nvcc, '-shared', '-o', OUT] + objs + ARCH + ['-ldl']
     if verbose:
         print(' '.join(cmd))
     subprocess.check_call(cmd)

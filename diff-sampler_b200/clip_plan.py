@@ -5,8 +5,8 @@ models/ldm/modules/encoders/modules.py:137-159 (`FrozenCLIPEmbedder.forward`: to
 The arithmetic is Hugging Face transformers' CLIP text tower (modeling_clip.py: CLIPTextEmbeddings, CLIPEncoderLayer, CLIPAttention with
 a causal mask, CLIPMLP with quick_gelu, final_layer_norm); oracle/clip_oracle.py restates it and is pinned to transformers' own module.
 
-Same executor and op set as the denoisers: every linear is the tcgen05 GEMM kernel (fp16x3 split operands, fp32 accumulation), the
-12-head causal attention is the fused attn3 kernel (csrc/attention.cu, causal=1), LayerNorm / quick-GELU / the embedding gather are
+Same executor and op set as the denoisers: every linear is the wgmma GEMM kernel (fp16x3 split operands, fp32 accumulation), the
+12-head causal attention is the fused attention kernel (csrc/attention.cu, causal=1), LayerNorm / quick-GELU / the embedding gather are
 the HBM-bound companions.  Rows are the B x 77 tokens (77 is not a multiple of the 128-row tile: TMA zero-fills the ragged tiles and
 the epilogue masks them).  The tokenizer is caller-side (vocabulary files): the plan starts at int32 token ids.
 

@@ -1,20 +1,17 @@
-// Fused softmax attention for sm_100a (head dim padded to 64): O = softmax(scale * Q K^T) V without materialising the L x Lk
+// Fused softmax attention for sm_90a (head dim padded to 64): O = softmax(scale * Q K^T) V without materialising the L x Lk
 // score matrix in HBM.  Reference: diff-solvers-main/models/networks_edm.py:105-118 (AttentionOp) / :174-178 (UNetBlock attention),
 // models/ldm/modules/attention.py:152-196 (CrossAttention.forward).
 //
-// One CTA per (sample, head, 128-query tile); keys/values stream through in blocks of 128:
+// One CTA per (sample, head, 128-query tile); keys/values stream through in blocks of 64:
 //
-//   warp 0      TMA producer   Q tile once; K_j [128 keys x 64] and V_j^T [64 x 128 keys] (fp16 hi/lo planes) into 2-stage rings
-//   warp 1      MMA issuer     S_j = Q K_j^T  (3 split-precision passes, 128x128x16 tcgen05.mma, two S buffers in TMEM)
-//                              O_j = P_j V_j  (3 passes, 128x64x16, fresh TMEM accumulator per block)
-//   warps 2..9  softmax        one query row and one half (64 keys) of the block per thread: running max / sum, p = exp2(s - m)
-//                              split into fp16 hi/lo and written to shared memory in the 128B-swizzled K-major layout the MMA
-//                              reads; the running output lives in registers (O = alpha * O + O_j), so the TMEM accumulator
-//                              never needs rescaling.
+//   warpgroup 0      TMA producer (warp 0)  Q tile once; K_j [64 keys x 64] and V_j^T [64 x 64 keys] (fp16 hi/lo planes) into a ring
+//   warpgroups 1, 2  queries 0..63 / 64..127 of the tile, each on its own:
+//                    S_j = Q K_j^T   (3 split-precision passes of 64 x 64 x 16 wgmma, A and B from shared memory)
+//                    online softmax in registers (running max / sum per row, p = exp2(s * scale * log2 e - m))
+//                    O  += P_j V_j   (3 passes of 64 x 64 x 16 wgmma with P as the register A operand: the accumulator fragment of S
+//                                     is the A fragment of the next product, so P never leaves registers)
 //
-// QK^T of block j+1 is issued before the softmax of block j finishes (two S buffers); the softmax row-max pass of block j+1
-// overlaps P_j V_j.  Same split-precision contract as the GEMM kernel: Q, K, V and P are fp16 hi + lo planes, products are
-// hi*hi + lo*hi + hi*lo in fp32.
+// Same split-precision contract as the GEMM kernel: Q, K, V and P are fp16 hi + lo planes, products are hi*hi + lo*hi + hi*lo in fp32.
 #include "ops.h"
 #include "ptx.cuh"
 #include <cuda_fp16.h>
@@ -26,15 +23,15 @@ namespace dsb {
 
 int encode_map(CUtensorMap* m, const void* ptr, int rank, const int64_t* dims, const int64_t* strides_bytes, const int32_t* box);
 
-static constexpr int kAttnThreads = 320;            // warp 0 TMA, warp 1 MMA, warps 2..9 softmax
+static constexpr int kAttnThreads = 384;            // warpgroup 0: producer (warp 0), 1 and 2: 64 queries each
+static constexpr int kAttnStages = 4;
 static constexpr int kQBytes = 2 * 16384;          // Q hi, lo: 128 rows x 64 fp16 each
-static constexpr int kKStage = 2 * 16384;          // K hi, lo: 128 keys x 64 fp16
-static constexpr int kVStage = 4 * 8192;           // V^T [plane][key block of 64]: 64 d-rows x 64 keys fp16
-static constexpr int kPBytes = 4 * 16384;          // P [plane][key block of 64]: 128 rows x 64 keys fp16
-static constexpr int kOffK = kQBytes;
-static constexpr int kOffV = kOffK + 2 * kKStage;
-static constexpr int kOffP = kOffV + 2 * kVStage;
-static constexpr int kOffCtl = kOffP + kPBytes;    // 224 KB
+static constexpr int kKBytes = 2 * 8192;           // K hi, lo: 64 keys x 64 fp16
+static constexpr int kVBytes = 2 * 8192;           // V^T hi, lo: 64 d-rows x 64 keys fp16
+static constexpr int kStageBytes = kKBytes + kVBytes;
+static constexpr int kOffKV = kQBytes;
+static constexpr int kOffCtl = kOffKV + kAttnStages * kStageBytes;
+static constexpr size_t kAttnSmem = kOffCtl + 256 + 1024;
 
 struct alignas(64) AttnKernelParams {
     CUtensorMap tmQ, tmK, tmV;
@@ -43,40 +40,12 @@ struct alignas(64) AttnKernelParams {
     __half* out;
     long long o_plane;
     int o_pitch;
-    // debug timeline (ds_debug_attn_trace): CTA 0 records (tag << 40 | clock) for its first tiles; NULL in normal runs
-    unsigned long long* trace;
-    int trace_cap;
-    int interleave;             // attn3: issue the MMAs of P.V(j) and of the next score product alternately (two independent accumulation chains)
-    int causal;                 // attn3: query l sees keys <= l
-};
-
-// trace tags: who (0 TMA, 1 MMA, 2 + g softmax group g) << 16 | event << 8 | block index (low 8 bits).  Every role writes its own region
-// of the buffer through a private counter: one plain store + one clock read per event (an atomic slot allocation costs a round trip to
-// L2, ~900 cycles, which would drown the waits being measured).
-struct AttnTracer {
-    unsigned long long* base;
-    unsigned n, cap;
-    __device__ __forceinline__ AttnTracer(const AttnKernelParams& p, int who) {
-        const int per = p.trace ? p.trace_cap / 8 : 0;
-        base = (p.trace && blockIdx.x == 0 && (threadIdx.x & 31) == 0) ? p.trace + (long long)who * per : nullptr;
-        n = 1;
-        cap = per;
-    }
-    __device__ __forceinline__ void operator()(unsigned it, int who, int ev, int j) {
-        if (base && it < 2 && n < cap) {
-            base[n] = ((unsigned long long)((who << 16) | (ev << 8) | (j & 255) | (it << 20)) << 40) | (clock64() & 0xFFFFFFFFFFULL);
-            base[0] = ++n;                       // events written + 1
-        }
-    }
+    int causal;                 // query l sees keys <= l
 };
 
 struct AttnCtl {
     uint64_t q_full;
-    uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2];
-    uint64_t s_full[2], s_empty[2];
-    uint64_t p_full, o_full, o_empty;
-    uint32_t tmem_base;
-    float xch[2][128];          // row maximum / row sum exchange between the two key halves of a row
+    uint64_t kv_full[kAttnStages], kv_empty[kAttnStages];
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -85,1215 +54,177 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
+__device__ __forceinline__ void split_half2(float a, float b, uint32_t& hi, uint32_t& lo) {
+    const __half2 h2 = __floats2half2_rn(a, b);
+    const float2 hf = __half22float2(h2);
+    const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
+    hi = *reinterpret_cast<const uint32_t*>(&h2);
+    lo = *reinterpret_cast<const uint32_t*>(&l2);
+}
+
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_constant__ AttnKernelParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     AttnCtl* ctl = reinterpret_cast<AttnCtl*>(smem + kOffCtl);
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int qt = blockIdx.x % p.q_tiles;
     const int z = blockIdx.x / p.q_tiles;
     const int h = z % p.nh;
     const int b = z / p.nh;
-    const int nkv = (p.Lk + 127) >> 7;
+    // causal: the tile's last query sees keys up to qt * 128 + 127
+    const int lk_eff = p.causal ? min(p.Lk, qt * 128 + 128) : p.Lk;
+    const int nkv = (lk_eff + 63) >> 6;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmQ);
         tma_prefetch_desc(&p.tmK);
         tma_prefetch_desc(&p.tmV);
         mbar_init(&ctl->q_full, 1);
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&ctl->k_full[s], 1);
-            mbar_init(&ctl->k_empty[s], 1);
-            mbar_init(&ctl->v_full[s], 1);
-            mbar_init(&ctl->v_empty[s], 1);
-            mbar_init(&ctl->s_full[s], 1);
-            mbar_init(&ctl->s_empty[s], 8);
+        for (int s = 0; s < kAttnStages; ++s) {
+            mbar_init(&ctl->kv_full[s], 1);
+            mbar_init(&ctl->kv_empty[s], 2);                              // one arrival per query warpgroup
         }
-        mbar_init(&ctl->p_full, 8);
-        mbar_init(&ctl->o_full, 1);
-        mbar_init(&ctl->o_empty, 8);
         fence_barrier_init();
-    } else if (warp == 1) {
-        tmem_alloc(&ctl->tmem_base, 512);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ctl->tmem_base;
-    // TMEM columns: S buffers at 0 and 128, per-block P.V result at 256 (64 columns)
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
             mbar_arrive_expect_tx(&ctl->q_full, kQBytes);
             tma_load_3d(&p.tmQ, &ctl->q_full, smem, p.q_c0 + h * 64, qt * 128, b);
             tma_load_3d(&p.tmQ, &ctl->q_full, smem + 16384, p.q_c0 + h * 64, qt * 128, p.B + b);
             for (int j = 0; j < nkv; ++j) {
-                const int s = j & 1;
-                const uint32_t ph = (j >> 1) & 1;
-                mbar_wait(&ctl->k_empty[s], ph ^ 1);
-                mbar_arrive_expect_tx(&ctl->k_full[s], kKStage);
-                uint8_t* sk = smem + kOffK + s * kKStage;
-                tma_load_3d(&p.tmK, &ctl->k_full[s], sk, p.k_c0 + h * 64, j * 128, b);
-                tma_load_3d(&p.tmK, &ctl->k_full[s], sk + 16384, p.k_c0 + h * 64, j * 128, p.B + b);
-                mbar_wait(&ctl->v_empty[s], ph ^ 1);
-                mbar_arrive_expect_tx(&ctl->v_full[s], kVStage);
-                uint8_t* sv = smem + kOffV + s * kVStage;
-#pragma unroll
-                for (int pl = 0; pl < 2; ++pl)
-#pragma unroll
-                    for (int kb = 0; kb < 2; ++kb)
-                        tma_load_3d(&p.tmV, &ctl->v_full[s], sv + pl * 16384 + kb * 8192, j * 128 + kb * 64, h * 64, pl * p.B + b);
+                const int s = j % kAttnStages;
+                const uint32_t ph = (j / kAttnStages) & 1;
+                mbar_wait(&ctl->kv_empty[s], ph ^ 1);
+                mbar_arrive_expect_tx(&ctl->kv_full[s], kStageBytes);
+                uint8_t* sk = smem + kOffKV + s * kStageBytes;
+                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk, p.k_c0 + h * 64, j * 64, b);
+                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk + 8192, p.k_c0 + h * 64, j * 64, p.B + b);
+                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes, j * 64, h * 64, b);
+                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes + 8192, j * 64, h * 64, p.B + b);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc_s = umma_idesc_f16(128);
-            const uint32_t idesc_o = umma_idesc_f16(64);
-            const uint32_t sq = smem_u32(smem);
-            const uint32_t sp = smem_u32(smem + kOffP);
-            auto issue_qk = [&](int j) {
-                const int s = j & 1;
-                const uint32_t ph = (j >> 1) & 1;
-                mbar_wait(&ctl->k_full[s], ph);
-                mbar_wait(&ctl->s_empty[s], ph ^ 1);
-                tc_fence_after();
-                const uint32_t sk = smem_u32(smem + kOffK + s * kKStage);
-                const uint32_t d_tmem = tmem_base + s * 128;
-#pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {
-                    const uint64_t da = umma_desc_sw128(sq + (pass == 1 ? 16384 : 0));
-                    const uint64_t db = umma_desc_sw128(sk + (pass == 2 ? 16384 : 0));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc_s, (pass > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&ctl->k_empty[s]);
-                umma_commit(&ctl->s_full[s]);
-            };
-            mbar_wait(&ctl->q_full, 0);
-            issue_qk(0);
-            for (int j = 0; j < nkv; ++j) {
-                if (j + 1 < nkv) issue_qk(j + 1);
-                const int s = j & 1;
-                mbar_wait(&ctl->v_full[s], (j >> 1) & 1);
-                mbar_wait(&ctl->o_empty, (j & 1) ^ 1);        // softmax warps have read the previous block's P.V result
-                mbar_wait(&ctl->p_full, j & 1);
-                tc_fence_after();
-                const uint32_t sv = smem_u32(smem + kOffV + s * kVStage);
-                const uint32_t d_tmem = tmem_base + 256;
-#pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {
-                    const uint32_t a_pl = sp + (pass == 1 ? 32768 : 0);
-                    const uint32_t b_pl = sv + (pass == 2 ? 16384 : 0);
-#pragma unroll
-                    for (int kb = 0; kb < 2; ++kb) {
-                        const uint64_t da = umma_desc_sw128(a_pl + kb * 16384);
-                        const uint64_t db = umma_desc_sw128(b_pl + kb * 8192);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc_o, (pass > 0 || kb > 0 || k > 0) ? 1u : 0u);
-                    }
-                }
-                umma_commit(&ctl->v_empty[s]);
-                umma_commit(&ctl->o_full);
-            }
-        }
-    } else {
-        // Eight softmax warps: warps w and w + 4 share a TMEM lane quadrant (w % 4); each thread owns one query row and one HALF of
-        // the block's 128 keys (half = key block of 64) plus the matching 32 output columns.  Two warps per scheduler hide each
-        // other's latencies; the halves meet once per block (row maximum, through shared memory + a named barrier).
-        const int quad = warp & 3;                      // TMEM lane quadrant this warp may access
-        const int half = (warp - 2) >> 2;               // 0: warps 2..5, 1: warps 6..9
-        const int row = quad * 32 + lane;               // query row inside the tile
-        const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-        uint8_t* sP = smem + kOffP + half * 16384;
-        float m = -INFINITY, l = 0.f;
-        float O[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) O[i] = 0.f;
-        auto add_block_output = [&]() {
-            uint32_t v[32];
-            DSB_TMEM_LD_32(t_row + 256 + half * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) O[i] += __uint_as_float(v[i]);
-        };
-        for (int j = 0; j < nkv; ++j) {
-            const int sb = j & 1;
-            mbar_wait(&ctl->s_full[sb], (j >> 1) & 1);
-            tc_fence_after();
-            const int kvalid = p.Lk - j * 128 - half * 64;   // keys of this thread's half that exist (>= 64: all)
-            const uint32_t t_s = t_row + sb * 128 + half * 64;
-            // pass 1: maximum over this thread's 64 keys (four independent chains, second chunk requested early)
-            float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-            {
-                uint32_t v[2][32];
-                DSB_TMEM_LD_32(t_s, v[0]);
-                tmem_ld_wait();
-                DSB_TMEM_LD_32(t_s + 32, v[1]);
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    if (kvalid >= 64) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[c][i]));
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i)
-                            if (c * 32 + i < kvalid) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[c][i]));
-                    }
-                    if (c == 0) tmem_ld_wait();
-                }
-            }
-            const float mx_own = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-            // meet the other half of the row.  Slots alternate with the block parity so that one barrier per block is enough:
-            // the slot written in block j is next overwritten (by the partner) in block j + 1, after this thread has read it.
-            ctl->xch[half ^ (j & 1)][row] = mx_own;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            const float mx = fmaxf(mx_own, ctl->xch[(half ^ 1) ^ (j & 1)][row]);
-            const float m_new = fmaxf(m, mx * p.scale_log2e);
-            const float alpha = ex2_approx(m - m_new);  // first block: exp2(-inf) = 0
-            if (j > 0) {
-                // P_{j-1} V_{j-1} has completed: its result is readable and the P buffer is free again
-                mbar_wait(&ctl->o_full, (j - 1) & 1);
-                tc_fence_after();
-                add_block_output();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&ctl->o_empty);
-            }
-            if (alpha != 1.f) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) O[i] *= alpha;
-                l *= alpha;
-            }
-            // pass 2: p = exp2(s * scale * log2e - m), split into fp16 hi / lo (packed half2 conversions), swizzled K-major store
-            float l4[4] = {0.f, 0.f, 0.f, 0.f};
-            {
-                uint32_t v[2][32];
-                DSB_TMEM_LD_32(t_s, v[0]);
-                tmem_ld_wait();
-                DSB_TMEM_LD_32(t_s + 32, v[1]);
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int col = c * 32 + g * 8 + 2 * i;
-                            float p0 = ex2_approx(fmaf(__uint_as_float(v[c][g * 8 + 2 * i]), p.scale_log2e, -m_new));
-                            float p1 = ex2_approx(fmaf(__uint_as_float(v[c][g * 8 + 2 * i + 1]), p.scale_log2e, -m_new));
-                            if (kvalid < 64) {
-                                if (col >= kvalid) p0 = 0.f;
-                                if (col + 1 >= kvalid) p1 = 0.f;
-                            }
-                            l4[i] += p0 + p1;
-                            const __half2 h2 = __floats2half2_rn(p0, p1);
-                            const float2 hf = __half22float2(h2);
-                            const __half2 l2 = __floats2half2_rn(p0 - hf.x, p1 - hf.y);
-                            hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                            lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                        }
-                        const int chunk = c * 4 + g;                         // 16-byte chunk of the 128-byte row
-                        const uint32_t off = row * 128 + ((chunk ^ (row & 7)) << 4);
-                        *reinterpret_cast<uint4*>(sP + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4*>(sP + 32768 + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                    }
-                    if (c == 0) tmem_ld_wait();
-                }
-            }
-            l += (l4[0] + l4[1]) + (l4[2] + l4[3]);
-            m = m_new;
-            tc_fence_before();
-            fence_proxy_async();                        // generic-proxy smem writes -> visible to the tensor core (async proxy)
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&ctl->s_empty[sb]);
-                mbar_arrive(&ctl->p_full);
-            }
-        }
-        mbar_wait(&ctl->o_full, (nkv - 1) & 1);
-        tc_fence_after();
-        add_block_output();
-        // row sum: both halves
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        ctl->xch[half][row] = l;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        l += ctl->xch[half ^ 1][row];
-        const int grow = qt * 128 + row;
-        if (grow < p.L) {
-            const float inv = 1.f / l;
-            __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * 64 + half * 32;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                uint32_t hw[4], lw[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float a0 = O[g * 8 + 2 * i] * inv, a1 = O[g * 8 + 2 * i + 1] * inv;
-                    const __half2 h2 = __floats2half2_rn(a0, a1);
-                    const float2 hf = __half22float2(h2);
-                    const __half2 l2 = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
-                    hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                    lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                }
-                *reinterpret_cast<uint4*>(o + g * 8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                *reinterpret_cast<uint4*>(o + p.o_plane + g * 8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
-
-// ------------------------------------------------------------------------------------------ v2: persistent, two softmax groups
-// Round-2 kernel for 64-wide heads (default; DSB_ATTN_V1=1 selects the kernel above).  What changed, and why (ncu of the kernel above,
-// profiles/r01b_ncu_attention_sd15_L4096.txt: tensor pipe 33 %, no unit saturated -- the block period was the serial chain
-// PV_j -> softmax pass 2 of block j+1 -> PV_{j+1} through ONE P buffer, plus a per-block exchange between the two halves of a row):
-//   * key blocks of 64; TWO softmax groups of four warps (one warp per TMEM lane quadrant each) take alternate key blocks, each with its
-//     own P buffer and P.V accumulator, its own running (max, sum, output row) -- no exchange inside the key loop; the two partial results
-//     of a row are merged once per tile (the usual split-KV combine);
-//   * every group has TWO S accumulators in TMEM: the MMA warp keeps the scores of a group's NEXT block ready while the group is in its
-//     exponentials (issue order  QK(0..3) | PV(0) QK(4) | PV(1) QK(5) | ...), so a group never waits for the tensor pipe.  First version
-//     of this kernel (one S buffer per group, profiles/r02/ncu_attn2_v0_*.txt): 43 % of the softmax warps' samples were the wait for the
-//     next scores, tensor pipe 24 %;
-//   * the softmax walks its 64 scores in two chunks of 32 TMEM columns (no register spills: the v0 build spilled 136 bytes into the key
-//     loop and half of its stall samples were local-memory loads); key masking only in the partial last block;
-//   * persistent CTAs (grid = #SMs) walk the (sample, head, query tile) list: TMEM allocation, barrier set-up and descriptor prefetch happen
-//     once, and the loads / first QK products of the next tile run under the softmax tail and the combine of the current one;
-//   * K / V^T blocks go through rings (3 / 4 deep) that are not tied to a group.
-// Same operand contract as v1 (fp16 hi/lo planes, three MMA passes per product, fp32 accumulate, exact fp32 online softmax).
-static constexpr int kA2Threads = 320;              // warp 0 TMA, warp 1 MMA, warps 2..5 softmax group 0, warps 6..9 group 1
-static constexpr int kA2KRing = 3, kA2VRing = 4;
-static constexpr int kA2QBytes = 2 * 16384;         // Q hi, lo: 128 rows x 64 fp16
-static constexpr int kA2KStage = 2 * 8192;          // K block hi, lo: 64 keys x 64 fp16
-static constexpr int kA2VStage = 2 * 8192;          // V^T block hi, lo: 64 d-rows x 64 keys
-static constexpr int kA2PBuf = 2 * 16384;           // P hi, lo: 128 rows x 64 keys (one buffer per group)
-static constexpr int kA2OffK = kA2QBytes;
-static constexpr int kA2OffV = kA2OffK + kA2KRing * kA2KStage;
-static constexpr int kA2OffP = kA2OffV + kA2VRing * kA2VStage;
-static constexpr int kA2OffCtl = kA2OffP + 2 * kA2PBuf;          // 208 KB
-
-struct Attn2Ctl {
-    uint64_t q_full, q_empty;
-    uint64_t k_full[kA2KRing], k_empty[kA2KRing], v_full[kA2VRing], v_empty[kA2VRing];
-    uint64_t s_full[2][2], s_empty[2][2];   // [group][S slot]
-    uint64_t p_full[2], o_full[2], o_empty[2];
-    uint64_t x_full, x_empty;       // group 1 -> group 0 hand-over of the partial result of a tile (through P buffer 1)
-    uint32_t tmem_base;
-    float xm[128], xl[128];         // group 1's running max / sum per row
-};
-
-__device__ __forceinline__ void lds128(uint32_t saddr, uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d) {
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(saddr) : "memory");
-}
-__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
-template <bool MASKED>
-__device__ __forceinline__ void attn2_softmax_block(uint32_t t_s, uint32_t sP, int row, int kvalid, float scale_log2e, float& m, float& l,
-                                                    float (&O)[64], bool have, uint64_t* o_full_bar, uint32_t o_parity, uint32_t t_o,
-                                                    uint64_t* o_empty_bar, int lane) {
-    // pass 1: row maximum over the block's 64 keys, 32 TMEM columns at a time
-    float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        DSB_TMEM_LD_32(t_s + c * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-            if (!MASKED || c * 32 + i < kvalid) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[i]));
-    }
-    const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-    const float m_new = fmaxf(m, mx * scale_log2e);
-    const float alpha = ex2_approx(m - m_new);       // first block: exp2(-inf) = 0
-    if (have) {
-        // P.V of this group's previous block has completed: fold it in (scaled to the new maximum in the same pass), release the
-        // accumulator -- and with it the P buffer this block is about to overwrite
-        mbar_wait(o_full_bar, o_parity);
-        tc_fence_after();
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            DSB_TMEM_LD_32(t_o + c * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) O[c * 32 + i] = (O[c * 32 + i] + __uint_as_float(v[i])) * alpha;
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(o_empty_bar);
-        l *= alpha;
-    }
-    // pass 2: p = exp2(s * scale * log2e - m), split into fp16 hi / lo, swizzled K-major store (one 128-byte row per query and plane)
-    float l4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        DSB_TMEM_LD_32(t_s + c * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int q8 = 0; q8 < 4; ++q8) {
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int col = c * 32 + q8 * 8 + 2 * i;
-                float p0 = ex2_approx(fmaf(__uint_as_float(v[q8 * 8 + 2 * i]), scale_log2e, -m_new));
-                float p1 = ex2_approx(fmaf(__uint_as_float(v[q8 * 8 + 2 * i + 1]), scale_log2e, -m_new));
-                if (MASKED) {
-                    if (col >= kvalid) p0 = 0.f;
-                    if (col + 1 >= kvalid) p1 = 0.f;
-                }
-                l4[i] += p0 + p1;
-                const __half2 h2 = __floats2half2_rn(p0, p1);
-                const float2 hf = __half22float2(h2);
-                const __half2 l2 = __floats2half2_rn(p0 - hf.x, p1 - hf.y);
-                hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-            }
-            const int chunk = c * 4 + q8;                        // 16-byte chunk of the 128-byte row
-            const uint32_t off = row * 128 + ((chunk ^ (row & 7)) << 4);
-            sts128(sP + off, hw[0], hw[1], hw[2], hw[3]);
-            sts128(sP + 16384 + off, lw[0], lw[1], lw[2], lw[3]);
-        }
-    }
-    l += (l4[0] + l4[1]) + (l4[2] + l4[3]);
-    m = m_new;
-}
-
-__global__ void __launch_bounds__(kA2Threads, 1) attn2_kernel(const __grid_constant__ AttnKernelParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    Attn2Ctl* ctl = reinterpret_cast<Attn2Ctl*>(smem + kA2OffCtl);
-
-    const int warp = threadIdx.x >> 5;
+    // ---------------------------------------------------------------------- query warpgroups
+    const int cw = wg - 1;
     const int lane = threadIdx.x & 31;
-    const int nkv = (p.Lk + 63) >> 6;
-    const int n_tiles = p.B * p.nh * p.q_tiles;
+    const int w = (threadIdx.x >> 5) & 3;
+    const int r0 = cw * 64 + 16 * w + (lane >> 2);          // query rows r0 and r0 + 8 of the tile
+    const int q0 = qt * 128 + r0;
+    const uint32_t sq = smem_u32(smem) + cw * 64 * 128;
+    float O[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) O[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&p.tmQ);
-        tma_prefetch_desc(&p.tmK);
-        tma_prefetch_desc(&p.tmV);
-        mbar_init(&ctl->q_full, 1);
-        mbar_init(&ctl->q_empty, 1);
-        for (int s = 0; s < kA2KRing; ++s) {
-            mbar_init(&ctl->k_full[s], 1);
-            mbar_init(&ctl->k_empty[s], 1);
+    mbar_wait(&ctl->q_full, 0);
+    for (int j = 0; j < nkv; ++j) {
+        const int s = j % kAttnStages;
+        mbar_wait(&ctl->kv_full[s], (j / kAttnStages) & 1);
+        const uint32_t sk = smem_u32(smem + kOffKV + s * kStageBytes);
+        const uint32_t sv = sk + kKBytes;
+        float S[32];
+        wgmma_fence();
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+            const uint64_t da = wgmma_desc_sw128(sq + (pass == 1 ? 16384 : 0));
+            const uint64_t db = wgmma_desc_sw128(sk + (pass == 2 ? 8192 : 0));
+#pragma unroll
+            for (int k = 0; k < 4; ++k) Wgmma<64>::f16(S, da + 2 * k, db + 2 * k, (pass > 0 || k > 0) ? 1u : 0u);
         }
-        for (int s = 0; s < kA2VRing; ++s) {
-            mbar_init(&ctl->v_full[s], 1);
-            mbar_init(&ctl->v_empty[s], 1);
-        }
-        for (int g = 0; g < 2; ++g) {
-            for (int s = 0; s < 2; ++s) {
-                mbar_init(&ctl->s_full[g][s], 1);
-                mbar_init(&ctl->s_empty[g][s], 4);
-            }
-            mbar_init(&ctl->p_full[g], 4);
-            mbar_init(&ctl->o_full[g], 1);
-            mbar_init(&ctl->o_empty[g], 4);
-        }
-        mbar_init(&ctl->x_full, 4);
-        mbar_init(&ctl->x_empty, 4);
-        fence_barrier_init();
-    } else if (warp == 1) {
-        tmem_alloc(&ctl->tmem_base, 512);
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ctl->tmem_base;
-    // TMEM columns: S[g][slot] at 128 g + 64 slot (64 columns each), per-block P.V result O[g] at 256 + 64 g
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(S);
 
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
-            uint32_t kc = 0, vc = 0, it = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-                const int qt = tile % p.q_tiles;
-                const int z = tile / p.q_tiles;
-                const int h = z % p.nh, b = z / p.nh;
-                mbar_wait(&ctl->q_empty, (it & 1) ^ 1);
-                mbar_arrive_expect_tx(&ctl->q_full, kA2QBytes);
-                tma_load_3d(&p.tmQ, &ctl->q_full, smem, p.q_c0 + h * 64, qt * 128, b);
-                tma_load_3d(&p.tmQ, &ctl->q_full, smem + 16384, p.q_c0 + h * 64, qt * 128, p.B + b);
-                for (int j = 0; j < nkv; ++j) {
-                    const int ks = kc % kA2KRing;
-                    mbar_wait(&ctl->k_empty[ks], ((kc / kA2KRing) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&ctl->k_full[ks], kA2KStage);
-                    uint8_t* sk = smem + kA2OffK + ks * kA2KStage;
-                    tma_load_3d(&p.tmK, &ctl->k_full[ks], sk, p.k_c0 + h * 64, j * 64, b);
-                    tma_load_3d(&p.tmK, &ctl->k_full[ks], sk + 8192, p.k_c0 + h * 64, j * 64, p.B + b);
-                    ++kc;
-                    const int vs = vc % kA2VRing;
-                    mbar_wait(&ctl->v_empty[vs], ((vc / kA2VRing) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&ctl->v_full[vs], kA2VStage);
-                    uint8_t* sv = smem + kA2OffV + vs * kA2VStage;
-                    tma_load_3d(&p.tmV, &ctl->v_full[vs], sv, j * 64, h * 64, b);
-                    tma_load_3d(&p.tmV, &ctl->v_full[vs], sv + 8192, j * 64, h * 64, p.B + b);
-                    ++vc;
-                }
-            }
+        // S fragment: S[4 g + e] is row r0 + 8 (e >> 1), key j * 64 + 8 g + 2 (lane & 3) + (e & 1)
+        float mx[2] = {-INFINITY, -INFINITY};
+        int kv[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            int lim = p.Lk - j * 64;
+            if (p.causal) lim = min(lim, q0 + 8 * hr - j * 64 + 1);
+            kv[hr] = lim;                                     // keys of this block the row may see: column c valid iff c < kv
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_f16(64);
-            const uint32_t sq = smem_u32(smem);
-            uint32_t kc = 0, vc = 0, it = 0;
-            uint32_t sc0 = 0, sc1 = 0, pc0 = 0, pc1 = 0;    // S products / P.V products issued per group
-            auto issue_qk = [&](int j) {
-                const int g = j & 1;
-                const int ks = kc % kA2KRing;
-                const uint32_t scg = g ? sc1 : sc0;
-                const int slot = scg & 1;
-                mbar_wait(&ctl->k_full[ks], (kc / kA2KRing) & 1);
-                mbar_wait(&ctl->s_empty[g][slot], ((scg >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t sk = smem_u32(smem + kA2OffK + ks * kA2KStage);
-                const uint32_t d_tmem = tmem_base + g * 128 + slot * 64;
 #pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {
-                    const uint64_t da = umma_desc_sw128(sq + (pass == 1 ? 16384 : 0));
-                    const uint64_t db = umma_desc_sw128(sk + (pass == 2 ? 8192 : 0));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (pass > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&ctl->k_empty[ks]);
-                umma_commit(&ctl->s_full[g][slot]);
-                ++kc;
-                if (g) ++sc1; else ++sc0;
-            };
-            auto issue_pv = [&](int j) {
-                const int g = j & 1;
-                const int vs = vc % kA2VRing;
-                const uint32_t pcg = g ? pc1 : pc0;
-                mbar_wait(&ctl->v_full[vs], (vc / kA2VRing) & 1);
-                mbar_wait(&ctl->p_full[g], pcg & 1);
-                mbar_wait(&ctl->o_empty[g], (pcg & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t sv = smem_u32(smem + kA2OffV + vs * kA2VStage);
-                const uint32_t sp = smem_u32(smem + kA2OffP + g * kA2PBuf);
-                const uint32_t d_tmem = tmem_base + 256 + g * 64;
-#pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {
-                    const uint64_t da = umma_desc_sw128(sp + (pass == 1 ? 16384 : 0));
-                    const uint64_t db = umma_desc_sw128(sv + (pass == 2 ? 8192 : 0));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (pass > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&ctl->v_empty[vs]);
-                umma_commit(&ctl->o_full[g]);
-                ++vc;
-                if (g) ++pc1; else ++pc0;
-            };
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-                mbar_wait(&ctl->q_full, it & 1);
-                const int ahead = nkv < 4 ? nkv : 4;             // score products run two blocks ahead of each group
-                for (int j = 0; j < ahead; ++j) issue_qk(j);
-                if (nkv <= 4) umma_commit(&ctl->q_empty);        // all S products of this tile are issued: Q may be overwritten once they complete
-                for (int j = 0; j < nkv; ++j) {
-                    issue_pv(j);
-                    if (j + 4 < nkv) {
-                        issue_qk(j + 4);
-                        if (j + 5 == nkv) umma_commit(&ctl->q_empty);
-                    }
-                }
-            }
+        for (int i = 0; i < 32; ++i) {
+            const int hr = (i >> 1) & 1;
+            const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+            if (col < kv[hr]) mx[hr] = fmaxf(mx[hr], S[i]);
         }
-    } else {
-        // ------------------------------------------------------------------ softmax groups
-        const int g = (warp - 2) >> 2;                  // group 0: warps 2..5, group 1: warps 6..9
-        const int quad = warp & 3;                      // TMEM lane quadrant this warp may access
-        const int row = quad * 32 + lane;               // query row inside the tile
-        const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-        const uint32_t t_o = t_row + 256 + g * 64;
-        const uint32_t sP = smem_u32(smem + kA2OffP + g * kA2PBuf);
-        float* xO = reinterpret_cast<float*>(smem + kA2OffP + kA2PBuf);       // group 1's P buffer doubles as the hand-over area [64][128]
-        uint32_t bc = 0, it = 0;                        // key blocks processed by this group / tiles processed
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-            const int qt = tile % p.q_tiles;
-            const int z = tile / p.q_tiles;
-            const int h = z % p.nh, b = z / p.nh;
-            float m = -INFINITY, l = 0.f;
-            float O[64];
+        float alpha[2], mn[2];
 #pragma unroll
-            for (int i = 0; i < 64; ++i) O[i] = 0.f;
-            bool have = false;
-            for (int j = g; j < nkv; j += 2) {
-                if (g == 1 && !have) {
-                    // first write of this tile into P buffer 1: group 0 must have read the previous tile's hand-over out of it
-                    mbar_wait(&ctl->x_empty, (it & 1) ^ 1);
-                }
-                const int slot = bc & 1;
-                mbar_wait(&ctl->s_full[g][slot], (bc >> 1) & 1);
-                tc_fence_after();
-                const int kvalid = p.Lk - j * 64;        // keys of this block that exist (>= 64: all)
-                const uint32_t t_s = t_row + g * 128 + slot * 64;
-                if (kvalid >= 64)
-                    attn2_softmax_block<false>(t_s, sP, row, 64, p.scale_log2e, m, l, O, have, &ctl->o_full[g], (bc - 1) & 1, t_o, &ctl->o_empty[g], lane);
-                else
-                    attn2_softmax_block<true>(t_s, sP, row, kvalid, p.scale_log2e, m, l, O, have, &ctl->o_full[g], (bc - 1) & 1, t_o, &ctl->o_empty[g], lane);
-                have = true;
-                ++bc;
-                tc_fence_before();
-                fence_proxy_async();                    // generic-proxy smem writes -> visible to the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) {
-                    mbar_arrive(&ctl->s_empty[g][slot]);
-                    mbar_arrive(&ctl->p_full[g]);
-                }
-            }
-            if (have) {
-                // the last block's P.V
-                mbar_wait(&ctl->o_full[g], (bc - 1) & 1);
-                tc_fence_after();
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    uint32_t v[32];
-                    DSB_TMEM_LD_32(t_o + c * 32, v);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) O[c * 32 + i] += __uint_as_float(v[i]);
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&ctl->o_empty[g]);
-            }
-            // ---- merge the two groups' partial results of this tile (rows are independent: thread `row` of group 1 hands its row to
-            //      thread `row` of group 0) and write the output
-            if (nkv > 1) {
-                if (g == 1) {
-                    // `have` is true here (nkv > 1), so the wait on x_empty above has happened and P buffer 1 is ours
-                    ctl->xm[row] = m;
-                    ctl->xl[row] = l;
-#pragma unroll
-                    for (int i = 0; i < 64; ++i) xO[i * 128 + row] = O[i];
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&ctl->x_full);    // release: the stores above are visible to whoever acquires the phase
-                } else {
-                    mbar_wait(&ctl->x_full, it & 1);
-                    const float m1 = ctl->xm[row], l1 = ctl->xl[row];
-                    const float mc = fmaxf(m, m1);
-                    const float f0 = ex2_approx(m - mc), f1 = ex2_approx(m1 - mc);
-                    l = l * f0 + l1 * f1;
-#pragma unroll
-                    for (int i = 0; i < 64; ++i) O[i] = O[i] * f0 + xO[i * 128 + row] * f1;
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&ctl->x_empty);
-                }
-            }
-            if (g == 0) {
-                const int grow = qt * 128 + row;
-                if (grow < p.L) {
-                    const float inv = 1.f / l;
-                    __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * 64;
-#pragma unroll
-                    for (int q8 = 0; q8 < 8; ++q8) {
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float a0 = O[q8 * 8 + 2 * i] * inv, a1 = O[q8 * 8 + 2 * i + 1] * inv;
-                            const __half2 h2 = __floats2half2_rn(a0, a1);
-                            const float2 hf = __half22float2(h2);
-                            const __half2 l2 = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
-                            hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                            lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                        }
-                        *reinterpret_cast<uint4*>(o + q8 * 8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4*>(o + p.o_plane + q8 * 8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                    }
-                }
-            }
+        for (int hr = 0; hr < 2; ++hr) {
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+            mn[hr] = fmaxf(m[hr], mx[hr] * p.scale_log2e);
+            // a row that has seen no key yet keeps m = -inf: its weights are all zero (masked), nothing to rescale
+            alpha[hr] = mn[hr] == -INFINITY ? 1.f : ex2_approx(m[hr] - mn[hr]);
         }
+        uint32_t Ph[16], Pl[16];
+        float ls[2] = {0.f, 0.f};
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+            const int hr = (i >> 1) & 1;
+            const int col = 8 * (i >> 2) + 2 * (lane & 3);
+            const float p0 = col < kv[hr] ? ex2_approx(fmaf(S[i], p.scale_log2e, -mn[hr])) : 0.f;
+            const float p1 = col + 1 < kv[hr] ? ex2_approx(fmaf(S[i + 1], p.scale_log2e, -mn[hr])) : 0.f;
+            ls[hr] += p0 + p1;
+            split_half2(p0, p1, Ph[i >> 1], Pl[i >> 1]);
+        }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            l[hr] = l[hr] * alpha[hr] + ls[hr];
+            m[hr] = mn[hr];
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) O[i] *= alpha[(i >> 1) & 1];
+
+        // O += P V: k-chunk kc (keys 16 kc .. +15) of P is S registers 8 kc .. 8 kc + 7, i.e. Ph / Pl [4 kc .. 4 kc + 3]
+        wgmma_fence();
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+            const uint32_t* A = pass == 1 ? Pl : Ph;
+            const uint64_t db = wgmma_desc_sw128(sv + (pass == 2 ? 8192 : 0));
+#pragma unroll
+            for (int kc = 0; kc < 4; ++kc) wgmma_f16_rs_n64(O, A + 4 * kc, db + 2 * kc);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(O);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&ctl->kv_empty[s]);
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
-
-// ------------------------------------------------------------------------------------------ v3: four softmax groups, output in TMEM
-// ncu of v2 (profiles/r02/ncu_attn2_v1_imagenet64_L1024.txt): tensor pipe 29 %, issue slots 32 % busy, 43 % of the softmax warps' samples in
-// ONE wait -- for the P.V product of their previous block, which they need (a) to fold into the register-resident output row and (b) before
-// they may overwrite their P buffer.  With two warps per scheduler nothing covers that wait, and the exponentials (~8 instructions per
-// score: scale, ex2, sum, fp16 hi/lo split) cannot reach one instruction per cycle.  v3 changes the division of labour:
-//   * FOUR softmax groups (16 warps, one per TMEM lane quadrant and group; blocks j = g, g + 4, ...): four warps per scheduler cover each
-//     other's waits and dependency stalls;
-//   * the running output row stays in TMEM: P.V accumulates across a group's blocks (tcgen05.mma accumulate), so the softmax warps no longer
-//     read 64 output columns per block.  The usual rescaling by exp2(m_old - m_new) is LAZY: a row keeps exponentiating against its
-//     current reference maximum until a block's maximum exceeds it by more than 8 (p <= 2^8: harmless for the fp16 hi/lo split, exact
-//     for the final O / l); only then -- a warp vote -- the group rescales its accumulator in place (tcgen05.ld -> multiply -> tcgen05.st);
-//   * per thread that leaves: row maximum (FMNMX3), p = ex2(s * scale - m), the sum, the hi/lo split and the swizzled stores -- ~6
-//     instructions per score and ~75 live registers, which is what lets 18 warps fit the register file (112 registers per thread);
-//   * one S accumulator per group (4 x 64 TMEM columns) + one output accumulator per group (4 x 64): all 512 columns; K / V rings two deep
-//     with the K loads running two blocks ahead of the V loads; P buffers 4 x 32 KB: 224 KB of shared memory in all;
-//   * the four partial results of a row are merged at the end of a tile in normalised form (O_g / l_g and lambda_g = m_g + log2 l_g).
-// NG softmax groups: 4 (K / V rings two deep) or 3 (rings three deep) -- the same 224 KB either way; DSB_ATTN_GROUPS selects (default below).
-template <int NG> struct A3 {
-    static constexpr int kThreads = 64 + NG * 128;             // warp 0 TMA, warp 1 MMA, then four warps per softmax group
-    static constexpr int kRing = NG == 4 ? 2 : 3;
-    static constexpr int kOffK = kA2QBytes;
-    static constexpr int kOffV = kOffK + kRing * kA2KStage;
-    static constexpr int kOffP = kOffV + kRing * kA2VStage;
-    static constexpr int kOffCtl = kOffP + NG * kA2PBuf;      // 224 KB
-};
-static constexpr float kA3RescaleThreshold = 8.0f;
-
-template <int NG> struct Attn3Ctl {
-    uint64_t q_full, q_empty;
-    uint64_t k_full[A3<NG>::kRing], k_empty[A3<NG>::kRing], v_full[A3<NG>::kRing], v_empty[A3<NG>::kRing];
-    uint64_t s_full[NG], s_empty[NG], p_full[NG], o_full[NG], o_empty[NG];
-    uint64_t x_full[NG], x_empty[NG];
-    uint64_t qt_full, qt_free;      // MODE 2: query tile copied into TMEM / all score products of the tile have read it
-    uint32_t tmem_base;
-    float xl[NG - 1][128];          // lambda = m + log2(l) of groups 1 .. NG - 1, per row
-};
-static constexpr int kA3SmemBytes = 227 * 1024;      // everything the SM has: 224 KB of tiles + the control block + alignment slack
-
-__device__ __forceinline__ float lg2_approx(float x) {
-    float y;
-    asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
-template <bool MASKED>
-__device__ __forceinline__ float attn3_row_max(uint32_t t_s, int kvalid) {
-    float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        DSB_TMEM_LD_32(t_s + c * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-            if (!MASKED || c * 32 + i < kvalid) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[i]));
+    for (int hr = 0; hr < 2; ++hr) {
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 1);
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
     }
-    return fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-}
-
-template <bool MASKED>
-__device__ __forceinline__ float attn3_exp_store(uint32_t t_s, uint32_t sP, int row, int kvalid, float scale_log2e, float m_ref) {
-    float l4[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        DSB_TMEM_LD_32(t_s + c * 32, v);
-        tmem_ld_wait();
+    for (int hr = 0; hr < 2; ++hr) {
+        const int grow = q0 + 8 * hr;
+        if (grow >= p.L) continue;
+        const float inv = 1.f / l[hr];
+        __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * 64 + 2 * (lane & 3);
 #pragma unroll
-        for (int q8 = 0; q8 < 4; ++q8) {
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int col = c * 32 + q8 * 8 + 2 * i;
-                float p0 = ex2_approx(fmaf(__uint_as_float(v[q8 * 8 + 2 * i]), scale_log2e, -m_ref));
-                float p1 = ex2_approx(fmaf(__uint_as_float(v[q8 * 8 + 2 * i + 1]), scale_log2e, -m_ref));
-                if (MASKED) {
-                    if (col >= kvalid) p0 = 0.f;
-                    if (col + 1 >= kvalid) p1 = 0.f;
-                }
-                l4[i] += p0 + p1;
-                const __half2 h2 = __floats2half2_rn(p0, p1);
-                const float2 hf = __half22float2(h2);
-                const __half2 l2 = __floats2half2_rn(p0 - hf.x, p1 - hf.y);
-                hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-            }
-            const int chunk = c * 4 + q8;                        // 16-byte chunk of the 128-byte row
-            const uint32_t off = row * 128 + ((chunk ^ (row & 7)) << 4);
-            sts128(sP + off, hw[0], hw[1], hw[2], hw[3]);
-            sts128(sP + 16384 + off, lw[0], lw[1], lw[2], lw[3]);
+        for (int g = 0; g < 8; ++g) {
+            uint32_t hi, lo;
+            split_half2(O[4 * g + 2 * hr] * inv, O[4 * g + 2 * hr + 1] * inv, hi, lo);
+            *reinterpret_cast<uint32_t*>(o + 8 * g) = hi;
+            *reinterpret_cast<uint32_t*>(o + p.o_plane + 8 * g) = lo;
         }
     }
-    return (l4[0] + l4[1]) + (l4[2] + l4[3]);
-}
-
-// P in tensor memory (PT variant): the probabilities replace the scores they were computed from.  Scores of keys 32 c .. 32 c + 31 sit in
-// columns 32 c .. 32 c + 31 (fp32); their fp16 hi parts go to columns 32 c .. 32 c + 15 (two keys per column), the lo parts to
-// columns 32 c + 16 .. 32 c + 31: each 16-key K slice of the P.V product is 8 consecutive columns (A operand from TMEM).
-template <bool MASKED>
-__device__ __forceinline__ float attn3_exp_store_tmem(uint32_t t_s, int kvalid, float scale_log2e, float m_ref) {
-    float l4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-        uint32_t v[32], u[32];
-        DSB_TMEM_LD_32(t_s + c * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const int col = c * 32 + 2 * i;
-            float p0 = ex2_approx(fmaf(__uint_as_float(v[2 * i]), scale_log2e, -m_ref));
-            float p1 = ex2_approx(fmaf(__uint_as_float(v[2 * i + 1]), scale_log2e, -m_ref));
-            if (MASKED) {
-                if (col >= kvalid) p0 = 0.f;
-                if (col + 1 >= kvalid) p1 = 0.f;
-            }
-            l4[i & 3] += p0 + p1;
-            const __half2 h2 = __floats2half2_rn(p0, p1);
-            const float2 hf = __half22float2(h2);
-            const __half2 l2 = __floats2half2_rn(p0 - hf.x, p1 - hf.y);
-            u[i] = *reinterpret_cast<const uint32_t*>(&h2);
-            u[16 + i] = *reinterpret_cast<const uint32_t*>(&l2);
-        }
-        DSB_TMEM_ST_32(t_s + c * 32, u);
-    }
-    return (l4[0] + l4[1]) + (l4[2] + l4[3]);
-}
-
-// MODE 0: P through shared memory; 1: P in tensor memory (A operand of P.V from TMEM); 2: Q in tensor memory as well (NG = 3: columns
-// 192 .. 255 hold the query tile, hi parts in 192 .. 223, lo parts in 224 .. 255, two fp16 per column) -- then every MMA of the kernel
-// reads only its 2 KB B operand from shared memory.
-template <int NG, int MODE>
-__global__ void __launch_bounds__(A3<NG>::kThreads, 1) attn3_kernel(const __grid_constant__ AttnKernelParams p) {
-    constexpr bool PT = MODE >= 1, QT = MODE == 2;
-    static_assert(!QT || NG == 3, "the query tile in TMEM needs the 64 columns a fourth group would use");
-    constexpr int kA3Groups = NG, kA3Ring = A3<NG>::kRing;
-    constexpr int kA3OffK = A3<NG>::kOffK, kA3OffV = A3<NG>::kOffV, kA3OffP = A3<NG>::kOffP, kA3OffCtl = A3<NG>::kOffCtl;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    Attn3Ctl<NG>* ctl = reinterpret_cast<Attn3Ctl<NG>*>(smem + kA3OffCtl);
-    if (threadIdx.x == 0 && (smem - smem_raw) + kA3OffCtl + (int)sizeof(Attn3Ctl<NG>) > kA3SmemBytes) __trap();
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const int nkv = (p.Lk + 63) >> 6;
-    const int n_tiles = p.B * p.nh * p.q_tiles;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&p.tmQ);
-        tma_prefetch_desc(&p.tmK);
-        tma_prefetch_desc(&p.tmV);
-        mbar_init(&ctl->q_full, 1);
-        mbar_init(&ctl->q_empty, QT ? 4 : 1);         // MODE 2: released by the four warps that copied the tile into TMEM
-        mbar_init(&ctl->qt_full, 4);
-        mbar_init(&ctl->qt_free, 1);
-        for (int s = 0; s < kA3Ring; ++s) {
-            mbar_init(&ctl->k_full[s], 1);
-            mbar_init(&ctl->k_empty[s], 1);
-            mbar_init(&ctl->v_full[s], 1);
-            mbar_init(&ctl->v_empty[s], 1);
-        }
-        for (int g = 0; g < kA3Groups; ++g) {
-            mbar_init(&ctl->s_full[g], 1);
-            mbar_init(&ctl->s_empty[g], 4);
-            mbar_init(&ctl->p_full[g], 4);
-            mbar_init(&ctl->o_full[g], 1);
-            mbar_init(&ctl->o_empty[g], 4);
-            mbar_init(&ctl->x_full[g], 4);
-            mbar_init(&ctl->x_empty[g], 4);
-        }
-        fence_barrier_init();
-    } else if (warp == 1) {
-        tmem_alloc(&ctl->tmem_base, 512);
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ctl->tmem_base;
-    // TMEM columns: S[g] at 64 g, output accumulator O[g] at 256 + 64 g
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer
-        // K and V^T blocks are two independent streams (K is consumed by the score products, which run up to NG blocks ahead of the
-        // P.V products that consume V): the thread polls both rings without blocking on either, so a V stage that is still being read
-        // never holds back the K block the MMA warp is waiting for.
-        if (lane == 0) {
-            AttnTracer tr(p, 0);
-            uint32_t kc = 0, vc = 0, it = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-                const int qt = tile % p.q_tiles;
-                const int z = tile / p.q_tiles;
-                const int h = z % p.nh, b = z / p.nh;
-                mbar_wait(&ctl->q_empty, (it & 1) ^ 1);
-                mbar_arrive_expect_tx(&ctl->q_full, kA2QBytes);
-                tma_load_3d(&p.tmQ, &ctl->q_full, smem, p.q_c0 + h * 64, qt * 128, b);
-                tma_load_3d(&p.tmQ, &ctl->q_full, smem + 16384, p.q_c0 + h * 64, qt * 128, p.B + b);
-                int kj = 0, vj = 0;
-                long long t0 = clock64();
-                while (kj < nkv || vj < nkv) {
-                    bool progress = false;
-                    if (kj < nkv) {
-                        const int ks = kc % kA3Ring;
-                        if (mbar_try_wait(&ctl->k_empty[ks], ((kc / kA3Ring) & 1) ^ 1)) {
-                            tr(it, 0, 0, kj);
-                            mbar_arrive_expect_tx(&ctl->k_full[ks], kA2KStage);
-                            uint8_t* sk = smem + kA3OffK + ks * kA2KStage;
-                            tma_load_3d(&p.tmK, &ctl->k_full[ks], sk, p.k_c0 + h * 64, kj * 64, b);
-                            tma_load_3d(&p.tmK, &ctl->k_full[ks], sk + 8192, p.k_c0 + h * 64, kj * 64, p.B + b);
-                            ++kc; ++kj;
-                            progress = true;
-                        }
-                    }
-                    if (vj < nkv) {
-                        const int vs = vc % kA3Ring;
-                        if (mbar_try_wait(&ctl->v_empty[vs], ((vc / kA3Ring) & 1) ^ 1)) {
-                            tr(it, 0, 1, vj);
-                            mbar_arrive_expect_tx(&ctl->v_full[vs], kA2VStage);
-                            uint8_t* sv = smem + kA3OffV + vs * kA2VStage;
-                            tma_load_3d(&p.tmV, &ctl->v_full[vs], sv, vj * 64, h * 64, b);
-                            tma_load_3d(&p.tmV, &ctl->v_full[vs], sv + 8192, vj * 64, h * 64, p.B + b);
-                            ++vc; ++vj;
-                            progress = true;
-                        }
-                    }
-                    if (progress) t0 = clock64();
-                    else if (clock64() - t0 > 4000000000LL) __trap();      // bounded like mbar_wait: a protocol bug must not hang the GPU
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (whole warp converged; tcgen05 instructions elected)
-        {
-            const uint32_t idesc = umma_idesc_f16(64);
-            const uint32_t sq = smem_u32(smem);
-            AttnTracer tr(p, 1);
-            uint32_t kc = 0, vc = 0, it = 0;
-            uint32_t s_par = 0, p_par = 0;       // bit g: parity of group g's next S product / P.V product
-            auto issue_qk = [&](int j) {
-                const int g = j % kA3Groups;
-                const int ks = kc % kA3Ring;
-                const uint32_t par = (s_par >> g) & 1;
-                tr(it, 1, 0, j);
-                mbar_wait_warp(&ctl->k_full[ks], (kc / kA3Ring) & 1);
-                tr(it, 1, 1, j);
-                if (!PT) mbar_wait_warp(&ctl->s_empty[g], par ^ 1);      // PT: the P.V product that read P out of S[g] was issued earlier (pipeline order)
-                tr(it, 1, 2, j);
-                tc_fence_after();
-                const uint32_t sk = smem_u32(smem + kA3OffK + ks * kA2KStage);
-                const uint32_t d_tmem = tmem_base + g * 64;
-                __syncwarp();
-                if (elect_one()) {
-#pragma unroll
-                    for (int pass = 0; pass < 3; ++pass) {
-                        const uint64_t da = umma_desc_sw128(sq + (pass == 1 ? 16384 : 0));
-                        const uint64_t db = umma_desc_sw128(sk + (pass == 2 ? 8192 : 0));
-                        const uint32_t tq = tmem_base + 192 + (pass == 1 ? 32 : 0);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            if (QT) umma_f16_ts(d_tmem, tq + 8 * k, db + 2 * k, idesc, (pass > 0 || k > 0) ? 1u : 0u);
-                            else umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (pass > 0 || k > 0) ? 1u : 0u);
-                        }
-                    }
-                    umma_commit(&ctl->k_empty[ks]);
-                    umma_commit(&ctl->s_full[g]);
-                }
-                __syncwarp();
-                ++kc;
-                s_par ^= 1u << g;
-            };
-            auto issue_pv = [&](int j) {
-                const int g = j % kA3Groups;
-                const int vs = vc % kA3Ring;
-                const uint32_t par = (p_par >> g) & 1;
-                tr(it, 1, 4, j);
-                mbar_wait_warp(&ctl->v_full[vs], (vc / kA3Ring) & 1);
-                tr(it, 1, 5, j);
-                mbar_wait_warp(&ctl->p_full[g], par);
-                tr(it, 1, 6, j);
-                const bool first = j < kA3Groups;           // this group's first block of the tile: fresh accumulator
-                if (first) mbar_wait_warp(&ctl->o_empty[g], (it & 1) ^ 1);      // the group has read the previous tile's result out of it
-                tc_fence_after();
-                const uint32_t sv = smem_u32(smem + kA3OffV + vs * kA2VStage);
-                const uint32_t sp = smem_u32(smem + kA3OffP + g * kA2PBuf);
-                const uint32_t d_tmem = tmem_base + 256 + g * 64;
-                __syncwarp();
-                if (elect_one()) {
-#pragma unroll
-                    for (int pass = 0; pass < 3; ++pass) {
-                        const uint64_t da = umma_desc_sw128(sp + (pass == 1 ? 16384 : 0));
-                        const uint64_t db = umma_desc_sw128(sv + (pass == 2 ? 8192 : 0));
-                        const uint32_t ta = tmem_base + g * 64 + (pass == 1 ? 16 : 0);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint32_t acc = (pass > 0 || k > 0 || !first) ? 1u : 0u;
-                            if (PT) umma_f16_ts(d_tmem, ta + (k >> 1) * 32 + (k & 1) * 8, db + 2 * k, idesc, acc);
-                            else umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, acc);
-                        }
-                    }
-                    umma_commit(&ctl->v_empty[vs]);
-                    umma_commit(&ctl->o_full[g]);
-                }
-                __syncwarp();
-                tr(it, 1, 7, j);
-                ++vc;
-                p_par ^= 1u << g;
-            };
-            // P.V(j) and the score product of block j + NG in ONE issue sequence, their MMAs alternating: consecutive tcgen05.mma into the
-            // same accumulator form a dependent chain (timeline in profiles/r02: ~95 cycles per 128x64x16 MMA issued back to back into one
-            // accumulator, three times its tensor time), two chains into different accumulators overlap.
-            auto issue_pv_qk = [&](int j, int jq) {
-                const int g = j % kA3Groups, gq = jq % kA3Groups;          // jq = j + NG (same group), or j + NG - 1 (previous group) with P in TMEM
-                const int vs = vc % kA3Ring, ks = kc % kA3Ring;
-                const uint32_t ppar = (p_par >> g) & 1, spar = (s_par >> gq) & 1;
-                tr(it, 1, 4, j);
-                mbar_wait_warp(&ctl->v_full[vs], (vc / kA3Ring) & 1);
-                mbar_wait_warp(&ctl->p_full[g], ppar);
-                const bool first = j < kA3Groups;
-                if (first) mbar_wait_warp(&ctl->o_empty[g], (it & 1) ^ 1);
-                tr(it, 1, 6, j);
-                mbar_wait_warp(&ctl->k_full[ks], (kc / kA3Ring) & 1);
-                if (!PT) mbar_wait_warp(&ctl->s_empty[gq], spar ^ 1);
-                tr(it, 1, 2, jq);
-                tc_fence_after();
-                const uint32_t sv = smem_u32(smem + kA3OffV + vs * kA2VStage);
-                const uint32_t sp = smem_u32(smem + kA3OffP + g * kA2PBuf);
-                const uint32_t sk = smem_u32(smem + kA3OffK + ks * kA2KStage);
-                const uint32_t d_o = tmem_base + 256 + g * 64, d_s = tmem_base + gq * 64;
-                __syncwarp();
-                if (elect_one()) {
-#pragma unroll
-                    for (int pass = 0; pass < 3; ++pass) {
-                        const uint64_t pa = umma_desc_sw128(sp + (pass == 1 ? 16384 : 0));
-                        const uint64_t pb = umma_desc_sw128(sv + (pass == 2 ? 8192 : 0));
-                        const uint64_t qa = umma_desc_sw128(sq + (pass == 1 ? 16384 : 0));
-                        const uint64_t qb = umma_desc_sw128(sk + (pass == 2 ? 8192 : 0));
-                        const uint32_t ta = tmem_base + g * 64 + (pass == 1 ? 16 : 0);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint32_t acc = (pass > 0 || k > 0 || !first) ? 1u : 0u;
-                            if (PT) umma_f16_ts(d_o, ta + (k >> 1) * 32 + (k & 1) * 8, pb + 2 * k, idesc, acc);
-                            else umma_f16(d_o, pa + 2 * k, pb + 2 * k, idesc, acc);
-                            if (QT) umma_f16_ts(d_s, tmem_base + 192 + (pass == 1 ? 32 : 0) + 8 * k, qb + 2 * k, idesc, (pass > 0 || k > 0) ? 1u : 0u);
-                            else umma_f16(d_s, qa + 2 * k, qb + 2 * k, idesc, (pass > 0 || k > 0) ? 1u : 0u);
-                        }
-                    }
-                    umma_commit(&ctl->v_empty[vs]);
-                    umma_commit(&ctl->k_empty[ks]);
-                    umma_commit(&ctl->o_full[g]);
-                    umma_commit(&ctl->s_full[gq]);
-                }
-                __syncwarp();
-                tr(it, 1, 7, j);
-                ++vc; ++kc;
-                p_par ^= 1u << g;
-                s_par ^= 1u << gq;
-            };
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-                mbar_wait_warp(QT ? &ctl->qt_full : &ctl->q_full, it & 1);
-                // score products run `look` blocks ahead of the P.V products.  With P in TMEM the scores of block j + NG go where P(j) is
-                // read from, so an interleaved pair is (P.V(j), S(j + NG - 1)): the S buffer of the previous group, whose P.V was issued before.
-                const int look = (PT && p.interleave) ? kA3Groups - 1 : kA3Groups;
-                const int ahead = nkv < look ? nkv : look;
-                for (int j = 0; j < ahead; ++j) issue_qk(j);
-                if (nkv <= look) { __syncwarp(); if (elect_one()) umma_commit(QT ? &ctl->qt_free : &ctl->q_empty); __syncwarp(); }
-                for (int j = 0; j < nkv; ++j) {
-                    if (j + look < nkv) {
-                        if (p.interleave) {
-                            issue_pv_qk(j, j + look);
-                        } else {
-                            issue_pv(j);
-                            issue_qk(j + look);
-                        }
-                        if (j + look + 1 == nkv) { __syncwarp(); if (elect_one()) umma_commit(QT ? &ctl->qt_free : &ctl->q_empty); __syncwarp(); }
-                    } else {
-                        issue_pv(j);
-                    }
-                }
-            }
-        }
-    } else {
-        // ------------------------------------------------------------------ softmax groups
-        const int g = (warp - 2) >> 2;                  // group g: warps 2 + 4 g .. 5 + 4 g
-        const int quad = warp & 3;                      // TMEM lane quadrant this warp may access
-        const int row = quad * 32 + lane;               // query row inside the tile
-        const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-        const uint32_t t_s = t_row + g * 64;
-        const uint32_t t_o = t_row + 256 + g * 64;
-        const uint32_t sP = smem_u32(smem + kA3OffP + g * kA2PBuf);
-        float* xO = reinterpret_cast<float*>(smem + kA3OffP + g * kA2PBuf);     // this group's P buffer doubles as its hand-over area [64][128]
-        const int ng = nkv < kA3Groups ? nkv : kA3Groups;                       // groups that have blocks
-        AttnTracer tr(p, 2 + g);
-        uint32_t bc = 0, it = 0;                        // key blocks processed by this group / tiles processed
-        // MODE 2: the last group moves the query tile of tile t from its TMA landing area into TMEM (each thread its own row: the
-        // 128-byte rows are 128B-swizzled, 16-byte chunk c of row r sits at chunk position c ^ (r & 7)) and hands the area back.
-        auto copy_q = [&](uint32_t t) {
-            mbar_wait(&ctl->qt_free, (t & 1) ^ 1);      // every score product of the previous tile has completed
-            mbar_wait(&ctl->q_full, t & 1);
-            const uint32_t sq = smem_u32(smem);
-#pragma unroll
-            for (int pl = 0; pl < 2; ++pl) {
-                uint32_t v[32];
-#pragma unroll
-                for (int c = 0; c < 8; ++c)
-                    lds128(sq + pl * 16384 + row * 128 + ((c ^ (row & 7)) << 4), v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-                DSB_TMEM_ST_32(t_row + 192 + pl * 32, v);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&ctl->qt_full);
-                mbar_arrive(&ctl->q_empty);
-            }
-        };
-        if (QT && g == kA3Groups - 1 && (int)blockIdx.x < n_tiles) copy_q(0);
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-            const int qt = tile % p.q_tiles;
-            const int z = tile / p.q_tiles;
-            const int h = z % p.nh, b = z / p.nh;
-            float m_ref = -INFINITY, l = 0.f;
-            bool have = false;
-            for (int j = g; j < nkv; j += kA3Groups) {
-                if (g > 0 && !have) mbar_wait(&ctl->x_empty[g], (it & 1) ^ 1);   // group 0 has read the previous tile's hand-over out of P[g]
-                if (quad == 0 && lane == 0) tr(it, 2 + g, 0, j);
-                mbar_wait(&ctl->s_full[g], bc & 1);
-                if (quad == 0 && lane == 0) tr(it, 2 + g, 1, j);
-                tc_fence_after();
-                int kvalid = p.Lk - j * 64;              // keys of this block that exist (>= 64: all) ...
-                if (p.causal) {                          // ... and that this thread's query may attend to (<= 0: none)
-                    const int lim = qt * 128 + row - j * 64 + 1;
-                    kvalid = lim < kvalid ? lim : kvalid;
-                }
-                const bool all_keys = __all_sync(0xffffffffu, kvalid >= 64);
-                const float t = (all_keys ? attn3_row_max<false>(t_s, 64) : attn3_row_max<true>(t_s, kvalid)) * p.scale_log2e;
-                if (quad == 0 && lane == 0) tr(it, 2 + g, 2, j);
-                if (!have) {
-                    m_ref = t;                           // first block of the row in this group: exact maximum, nothing to rescale
-                } else {
-                    // the previous P.V of this group has completed: the P buffer may be overwritten and the accumulator is stable
-                    mbar_wait(&ctl->o_full[g], (bc - 1) & 1);
-                    tc_fence_after();
-                    const bool need = t > m_ref + kA3RescaleThreshold;
-                    if (__any_sync(0xffffffffu, need)) {
-                        const float m_new = need ? t : m_ref;
-                        const float alpha = need ? ex2_approx(m_ref - m_new) : 1.f;      // rows that keep their reference (possibly -inf: no key seen yet)
-#pragma unroll
-                        for (int c = 0; c < 2; ++c) {
-                            uint32_t v[32];
-                            DSB_TMEM_LD_32(t_o + c * 32, v);
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-                            DSB_TMEM_ST_32(t_o + c * 32, v);
-                        }
-                        tmem_st_wait();
-                        l *= alpha;
-                        m_ref = m_new;
-                    }
-                }
-                if (quad == 0 && lane == 0) tr(it, 2 + g, 3, j);
-                if (PT) {
-                    l += all_keys ? attn3_exp_store_tmem<false>(t_s, 64, p.scale_log2e, m_ref)
-                                  : attn3_exp_store_tmem<true>(t_s, kvalid, p.scale_log2e, m_ref);
-                    tmem_st_wait();
-                } else {
-                    l += all_keys ? attn3_exp_store<false>(t_s, sP, row, 64, p.scale_log2e, m_ref)
-                                  : attn3_exp_store<true>(t_s, sP, row, kvalid, p.scale_log2e, m_ref);
-                }
-                have = true;
-                ++bc;
-                if (quad == 0 && lane == 0) tr(it, 2 + g, 4, j);
-                tc_fence_before();
-                if (!PT) fence_proxy_async();           // generic-proxy smem writes -> visible to the tensor core (async proxy)
-                __syncwarp();
-                if (quad == 0 && lane == 0) tr(it, 2 + g, 5, j);
-                if (lane == 0) {
-                    if (!PT) mbar_arrive(&ctl->s_empty[g]);
-                    mbar_arrive(&ctl->p_full[g]);
-                }
-            }
-            if (QT && g == kA3Groups - 1 && tile + (int)gridDim.x < n_tiles) copy_q(it + 1);
-            if (!have) continue;                         // fewer key blocks than groups: nothing for this group in any tile
-            // ---- this group's result of the tile: O = accumulator / l relative to m_ref
-            float O[64];
-            mbar_wait(&ctl->o_full[g], (bc - 1) & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                uint32_t v[32];
-                DSB_TMEM_LD_32(t_o + c * 32, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) O[c * 32 + i] = __uint_as_float(v[i]);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&ctl->o_empty[g]);
-            // a row may have seen no key at all in this group's blocks (causal mask): it then carries weight 2^-inf = 0
-            const float inv = l > 0.f ? 1.f / l : 0.f;
-            float lam = l > 0.f ? m_ref + lg2_approx(l) : -INFINITY;       // this partial result carries weight 2^lam
-#pragma unroll
-            for (int i = 0; i < 64; ++i) O[i] *= inv;
-            if (g > 0) {
-                ctl->xl[g - 1][row] = lam;
-#pragma unroll
-                for (int i = 0; i < 64; ++i) xO[i * 128 + row] = O[i];
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&ctl->x_full[g]);     // release: the stores above are visible to whoever acquires the phase
-                continue;
-            }
-            // group 0 merges the partial results of groups 1 .. ng - 1 (normalised rows, weights 2^lambda) and writes the output
-            float wsum = 1.f;
-#pragma unroll 1
-            for (int og = 1; og < ng; ++og) {
-                mbar_wait(&ctl->x_full[og], it & 1);
-                const float lo = ctl->xl[og - 1][row];
-                const float ln = fmaxf(lam, lo);
-                const float fa = ex2_approx(lam - ln), fb = ex2_approx(lo - ln);
-                const float* src = reinterpret_cast<const float*>(smem + kA3OffP + og * kA2PBuf) + row;
-#pragma unroll
-                for (int i = 0; i < 64; ++i) O[i] = O[i] * fa + src[i * 128] * fb;
-                wsum = wsum * fa + fb;
-                lam = ln;
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&ctl->x_empty[og]);
-            }
-            const int grow = qt * 128 + row;
-            if (grow < p.L) {
-                const float winv = 1.f / wsum;
-                __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * 64;
-#pragma unroll
-                for (int q8 = 0; q8 < 8; ++q8) {
-                    uint32_t hw[4], lw[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float a0 = O[q8 * 8 + 2 * i] * winv, a1 = O[q8 * 8 + 2 * i + 1] * winv;
-                        const __half2 h2 = __floats2half2_rn(a0, a1);
-                        const float2 hf = __half22float2(h2);
-                        const __half2 l2 = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
-                        hw[i] = *reinterpret_cast<const uint32_t*>(&h2);
-                        lw[i] = *reinterpret_cast<const uint32_t*>(&l2);
-                    }
-                    *reinterpret_cast<uint4*>(o + q8 * 8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                    *reinterpret_cast<uint4*>(o + p.o_plane + q8 * 8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                }
-            }
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 // ------------------------------------------------------------------------------------------ host
-// kernel generation: 3 (default: four softmax groups, output in TMEM), 2 (two groups, output in registers), 1 (round 1).
-// DSB_ATTN=1|2|3 selects it for the process; DSB_ATTN_V1=1 is the round-2a spelling of DSB_ATTN=1.
-static int attn_version() {
-    static const int v = [] {
-        const char* e1 = getenv("DSB_ATTN_V1");
-        if (e1 && atoi(e1)) return 1;
-        const char* e = getenv("DSB_ATTN");
-        const int x = e ? atoi(e) : 3;
-        return (x >= 1 && x <= 3) ? x : 3;
-    }();
-    return v;
-}
-static bool attn_use_v1() { return attn_version() == 1; }
-
-static unsigned long long* g_attn_trace = nullptr;
-static int g_attn_trace_cap = 0;
-void attn_set_trace(unsigned long long* dev_buf, int capacity) { g_attn_trace = dev_buf; g_attn_trace_cap = capacity; }
-
 int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
     if (d->nplanes != 2 || d->B <= 0 || d->nh <= 0 || d->L <= 0 || d->Lk <= 0 || !(d->scale > 0.f)) return -30;
     if (d->q_pitch % 8 || d->k_pitch % 8 || d->vt_pitch % 8 || d->o_pitch % 8 || d->q_c0 % 8 || d->k_c0 % 8) return -31;
     if (d->q_c0 + d->nh * 64 > d->q_pitch || d->k_c0 + d->nh * 64 > d->k_pitch || d->nh * 64 > d->o_pitch || d->Lk > d->vt_pitch) return -32;
+    if (d->causal && d->L != d->Lk) return -40;                       // the causal mask is defined for self-attention only
     {
         const int64_t dims[3] = {d->q_pitch, d->L, (int64_t)2 * d->B};
         const int64_t str[2] = {(int64_t)d->q_pitch * 2, (int64_t)d->L * d->q_pitch * 2};
@@ -1303,7 +234,7 @@ int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
     {
         const int64_t dims[3] = {d->k_pitch, d->Lk, (int64_t)2 * d->B};
         const int64_t str[2] = {(int64_t)d->k_pitch * 2, (int64_t)d->Lk * d->k_pitch * 2};
-        const int32_t box[3] = {64, attn_use_v1() ? 128 : 64, 1};          // key block: 128 (v1) / 64 (v2)
+        const int32_t box[3] = {64, 64, 1};
         if (encode_map(&kp->tmK, d->k, 3, dims, str, box)) return -34;
     }
     {
@@ -1318,79 +249,24 @@ int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
     kp->out = reinterpret_cast<__half*>(d->out);
     kp->o_plane = (long long)d->B * d->L * d->o_pitch;
     kp->o_pitch = d->o_pitch;
-    kp->trace = g_attn_trace;
-    kp->trace_cap = g_attn_trace_cap;
-    static const int inter = [] { const char* e = getenv("DSB_ATTN_INTERLEAVE"); return e ? atoi(e) : 1; }();
-    kp->interleave = inter;
     kp->causal = d->causal ? 1 : 0;
-    if (d->causal && (attn_version() != 3 || d->L != d->Lk)) return -40;       // the causal mask exists in the attn3 kernel only (self-attention)
     return 0;
 }
 
 size_t attn_params_size() { return sizeof(AttnKernelParams); }
 
-template <int NG, int MODE>
-static int attn3_launch(const AttnKernelParams* kp, cudaStream_t stream) {
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return -39;
-    if (!attr_set[dev]) {
-        if (cudaFuncSetAttribute(attn3_kernel<NG, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kA3SmemBytes) != cudaSuccess) return -36;
-        cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-        attr_set[dev] = true;
-    }
-    const long long tiles = (long long)kp->B * kp->nh * kp->q_tiles;
-    if (tiles <= 0 || tiles > 0x7fffffffLL) return -37;
-    const int grid = (int)(tiles < sms[dev] ? tiles : sms[dev]);
-    attn3_kernel<NG, MODE><<<grid, A3<NG>::kThreads, kA3SmemBytes, stream>>>(*kp);
-    return cudaGetLastError() == cudaSuccess ? 0 : -38;
-}
-
-static int attn3_run(const AttnKernelParams* kp, cudaStream_t stream) {
-    static const int groups = [] { const char* e = getenv("DSB_ATTN_GROUPS"); const int x = e ? atoi(e) : 4; return x == 3 ? 3 : 4; }();
-    // DSB_ATTN_TMEM: 0 = P through shared memory, 1 = P in tensor memory, 2 = P and Q in tensor memory (three groups)
-    static const int tm = [] { const char* e = getenv("DSB_ATTN_TMEM"); return e ? atoi(e) : 2; }();
-    if (tm >= 2) return attn3_launch<3, 2>(kp, stream);
-    if (tm == 1) return groups == 3 ? attn3_launch<3, 1>(kp, stream) : attn3_launch<4, 1>(kp, stream);
-    return groups == 3 ? attn3_launch<3, 0>(kp, stream) : attn3_launch<4, 0>(kp, stream);
-}
-
-static int attn2_run(const AttnKernelParams* kp, cudaStream_t stream) {
-    static bool attr_set[64] = {};
-    static int sms[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return -39;
-    const size_t smem = kA2OffCtl + sizeof(Attn2Ctl) + 1024;
-    if (!attr_set[dev]) {
-        if (cudaFuncSetAttribute(attn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -36;
-        cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-        attr_set[dev] = true;
-    }
-    const long long tiles = (long long)kp->B * kp->nh * kp->q_tiles;
-    if (tiles <= 0 || tiles > 0x7fffffffLL) return -37;
-    const int grid = (int)(tiles < sms[dev] ? tiles : sms[dev]);
-    attn2_kernel<<<grid, kA2Threads, smem, stream>>>(*kp);
-    return cudaGetLastError() == cudaSuccess ? 0 : -38;
-}
-
 int attn_run(const AttnKernelParams* kp, cudaStream_t stream) {
-    if (attn_version() == 3) return attn3_run(kp, stream);
-    if (attn_version() == 2) return attn2_run(kp, stream);
     static bool attr_set[64] = {};                  // per device (cudaFuncSetAttribute is a per-device setting)
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) return -39;
-    const size_t smem = kOffCtl + sizeof(AttnCtl) + 1024;
     if (!attr_set[dev]) {
-        if (cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -36;
+        if (cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmem) != cudaSuccess) return -36;
         attr_set[dev] = true;
     }
     const long long grid = (long long)kp->B * kp->nh * kp->q_tiles;
     if (grid <= 0 || grid > 0x7fffffffLL) return -37;
-    attn_kernel<<<(unsigned)grid, kAttnThreads, smem, stream>>>(*kp);
+    attn_kernel<<<(unsigned)grid, kAttnThreads, kAttnSmem, stream>>>(*kp);
     return cudaGetLastError() == cudaSuccess ? 0 : -38;
 }
 

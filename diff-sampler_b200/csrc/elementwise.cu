@@ -74,8 +74,8 @@ __global__ void __launch_bounds__(1024) gn_finalize_kernel(ds_gn_finalize_desc d
     const int C = d.C0 + d.C1;
     if (d.quads0) {
         // partial rows: {sum, sumsq} per unit of u0 / u1 channels (4 = quads, 2 = pairs) -> w floats per 32-row slab.
-        // Thread (column, slab group): the 1024 threads split the sample's slabs SG ways (round 2: one thread per column walked all
-        // HW / 32 slabs alone, 35 us per launch at 64 x 64); the SG partials of a column are added in a fixed order (deterministic).
+        // Thread (column, slab group): the 1024 threads split the sample's slabs SG ways (one thread per column walking all HW / 32
+        // slabs alone is slow at 64 x 64); the SG partials of a column are added in a fixed order (deterministic).
         const int u0 = d.unit0 == 2 ? 2 : 4, u1 = d.unit1 == 2 ? 2 : 4;
         const int w0 = d.C0 / u0 * 2, w1 = d.C1 / u1 * 2;
         const int cols = w0 + w1;
@@ -152,8 +152,7 @@ __global__ void __launch_bounds__(1024) gn_finalize_kernel(ds_gn_finalize_desc d
 // Packed arithmetic (two values per instruction wherever the ISA has it): v * 2^A16 -> f16x2 convert -> clamp as half2 (a value beyond the fp16
 // range converts to inf and is clamped back: the same result as clamping first) -> hi byte plane straight from the half2
 // (cvt.e4m3x2.f16x2 of hi * 2^(HI8 - A16), exact: a power of two) -> lo = fma(hi, -2^(LO8 - A16), v * 2^LO8) = (v - hi / 2^A16) * 2^LO8 with
-// one rounding, as before.  7 instructions per value instead of 11 (gn_apply with this store was issue-bound: 41 instructions per element
-// with both outputs, profiles/r02/ncu_gn_apply_v3_cifar_r02m.txt).
+// one rounding.  7 instructions per value instead of 11 (gn_apply with this store is otherwise bound by instruction issue).
 __device__ __forceinline__ void f8_image_pair(float v0, float v1, uint32_t& hi16, unsigned short& lo8, unsigned short& hi8) {
     constexpr float kA16 = (float)(1 << DS_F8_SH_A16), kLo8 = (float)(1 << DS_F8_SH_LO8);
     constexpr float kLoA = (float)(1 << (DS_F8_SH_LO8 - DS_F8_SH_A16));
@@ -341,10 +340,10 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int p
     }
 }
 
-// The plain (RESAMPLE == 0) path, default since round 1 (DSB_GN_APPLY_V2=0 selects the older loop inside gn_apply_kernel<0> for A/B): the
+// The plain (RESAMPLE == 0) path (DSB_GN_APPLY_V2=0 selects the older loop inside gn_apply_kernel<0> for A/B): the
 // normalisation is folded to one FMA per element, y = x * a + b' with b' = b - mean * a (16 instead of 24 live coefficient registers), and
 // four pixels are processed per iteration so that eight 16-byte loads are in flight per thread (the two-pixel loop keeps ~49 KB per SM in
-// flight, about the minimum HBM needs).  Measured on the CIFAR-10 forward at batch 512: 10.7 -> 9.55 ms (profiles/r01d).
+// flight, about the minimum HBM needs).
 template <int NP>
 __device__ __forceinline__ void gn_v2_pixels(const ds_gn_apply_desc& d, const float* base, int pitch, long long n, int npix, int C, int c,
                                              long long plane, int po, int rows, bool norm, const float* a, const float* b, __half* oact,
@@ -436,9 +435,9 @@ __global__ void __launch_bounds__(512) gn_apply_v2_kernel(ds_gn_apply_desc d, in
     for (; po < p_end; po += rows) gn_v2_pixels<1>(d, base, pitch, n, npix, C, c, plane, po, rows, norm, a, b, oact, oraw);
 }
 
-// Round 2 (resample == 0 with precomputed coefficients, ds_gn_apply_desc.coef): the v2 inner loop inside a PERSISTENT, EVENLY SPLIT grid.
-// v2 launched one CTA per (sample, 16-pixels-per-thread chunk): 4096 CTAs over 148 x 8 slots = 3.46 waves (a 13 % tail), each thread
-// paying an fp64 mean / rsqrt prologue for 16 pixels of work -- 76 % of the copy bandwidth (DESIGN.md section 9).  Here the (sample, pixel
+// resample == 0 with precomputed coefficients (ds_gn_apply_desc.coef): the v2 inner loop inside a PERSISTENT, EVENLY SPLIT grid.
+// v2 launches one CTA per (sample, 16-pixels-per-thread chunk): a partial last wave, and each thread pays an fp64 mean / rsqrt
+// prologue for 16 pixels of work.  Here the (sample, pixel
 // row) space is cut into gridDim.x equal ranges (+-1 row), the grid is exactly the number of co-resident CTAs, and a thread fetches its
 // 16 coefficients (4 x 16 B, L2-resident table written by gn_finalize) only when its range crosses into another sample.
 __global__ void __launch_bounds__(256, 3) gn_apply_v3_kernel(ds_gn_apply_desc d, int nc8, int rows, int units_per_sample, long long total_units) {
@@ -454,9 +453,8 @@ __global__ void __launch_bounds__(256, 3) gn_apply_v3_kernel(ds_gn_apply_desc d,
     else { base0 = d.src1; pitch = d.C1; cc = c - d.C0; }
     __half* oact = reinterpret_cast<__half*>(d.out_act);
     __half* oraw = reinterpret_cast<__half*>(d.out_raw);
-    // r02s: with one contiguous range per CTA (round-2 v3) the 444 CTAs streamed through 444 x (2 sources + up to 5 output planes) distant
-    // 2 MB pages at once and the 3.2 GB concat layers (512 channels, 32x32, act + raw outputs) ran at 2.8 TB/s against 5.3 TB/s for the
-    // 1 GB layers.  Now the grid sweeps the tensor together: chunks of kChunk units (>= 8 pixel rows, never crossing a sample) are dealt
+    // With one contiguous range per CTA every CTA would stream through its own distant pages (2 sources + up to 5 output planes each),
+    // which slows the large concat layers.  Instead the grid sweeps the tensor together: chunks of kChunk units (>= 8 pixel rows, never crossing a sample) are dealt
     // round-robin, so at any time all CTAs work inside one ~30 MB window per stream; the coefficients are refetched only when the sample
     // changes.
     constexpr int kChunk = 8;
@@ -926,7 +924,7 @@ extern "C" int ds_gn_stats_launch(const ds_gn_stats_desc* d, cudaStream_t stream
     if (pix_per_cta < 64) pix_per_cta = 64;
     // small batches (latent diffusion: 16 samples): shorter pixel runs per CTA so that the grid still covers the SMs
     const int min_pix = by > 8 ? by : 8;
-    while (pix_per_cta > min_pix && (long long)((d->HW + pix_per_cta - 1) / pix_per_cta) * d->B < 148 * 4) pix_per_cta /= 2;
+    while (pix_per_cta > min_pix && (long long)((d->HW + pix_per_cta - 1) / pix_per_cta) * d->B < 132 * 4) pix_per_cta /= 2;
     const int chunks = (d->HW + pix_per_cta - 1) / pix_per_cta;
     gn_stats_kernel<<<dim3(chunks, d->B), dim3(bx, by), 0, stream>>>(*d, pix_per_cta);
     return ok();
@@ -974,7 +972,7 @@ extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream
     const int npix = Ho * Wo;
     // ~16 pixels per thread amortise the per-thread coefficient set-up; keep at least ~4 CTAs per SM in flight overall
     int pix_per_cta = rows * 16;
-    while (pix_per_cta > rows && (long long)((npix + pix_per_cta - 1) / pix_per_cta) * d->B < 148 * 4) pix_per_cta /= 2;
+    while (pix_per_cta > rows && (long long)((npix + pix_per_cta - 1) / pix_per_cta) * d->B < 132 * 4) pix_per_cta /= 2;
     const int chunks = (npix + pix_per_cta - 1) / pix_per_cta;
     dim3 grid(chunks, d->B);
     if (d->coef && d->resample == 0 && d->sums == nullptr && threads > 256) return -2;      // wider than 2048 channels: use the sums path

@@ -23,7 +23,6 @@ struct AttnKernelParams;
 int attn_build(const ds_attn_desc* d, AttnKernelParams* kp);
 int attn_run(const AttnKernelParams* kp, cudaStream_t stream);
 size_t attn_params_size();
-void attn_set_trace(unsigned long long* dev_buf, int capacity);
 }  // namespace dsb
 
 static thread_local std::string g_err;
@@ -132,7 +131,7 @@ static int launch_op(const ds_plan_op& op, const unsigned char* gemm_kp, cudaStr
 
 extern "C" {
 
-const char* ds_version(void) { return "diffsampler_b200 0.1 (sm_100a, tcgen05/TMA)"; }
+const char* ds_version(void) { return "diffsampler_b200 0.1 (sm_90a, wgmma/TMA)"; }
 const char* ds_last_error(void) { return g_err.c_str(); }
 
 int ds_weights_create(const void* host_blob, size_t bytes, ds_weights** out) {
@@ -478,11 +477,6 @@ int ds_amed_predict(const float* weights, const int* dims6, const float* bottlen
     NvtxRange nvtx_range("ds_amed_predict");
     int rc = ds_amed_predict_launch(weights, dims6, bottleneck, t_cur, t_next, scale_dir, scale_time, out4, B, static_cast<cudaStream_t>(stream));
     if (rc) return fail(rc, std::string("ds_amed_predict: launch failed: ") + cudaGetErrorString(cudaGetLastError()));
-    return 0;
-}
-
-int ds_debug_attn_trace(unsigned long long* dev_buf, int capacity) {
-    dsb::attn_set_trace(dev_buf, capacity);
     return 0;
 }
 

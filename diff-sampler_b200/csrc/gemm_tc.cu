@@ -1,22 +1,19 @@
-// tcgen05 implicit-GEMM convolution / GEMM for sm_100a.
+// wgmma implicit-GEMM convolution / GEMM for sm_90a.
 //
 // One persistent, warp-specialised kernel serves every contraction of the denoiser U-Net
 // (reference: diff-solvers-main/models/networks_edm.py:60-82 Conv2d, :105-118 AttentionOp,
 //  :174-178 qkv/proj): 3x3 and 1x1 convolutions over NHWC fp16 activations, the 1x1 skip
 // projection appended along K, and the batched Q.K^T / P.V products of self-attention.
 //
-//   warp 0      TMA producer   (cp.async.bulk.tensor 4-D boxes for A = shifted pixel tiles / row-reuse halo boxes, 3-D for B)
-//   warp 1      MMA issuer     (tcgen05.mma kind::f16, 128 x BN x 16, fp32 accumulators in TMEM; in f8 mode the two split-precision
-//                               correction products are kind::f8f6f4 e4m3 MMAs, 128 x BN x 32, into the same accumulator)
-//   warps 2..9  epilogue       (two groups of four warps on alternate 32-column chunks: tcgen05.ld -> bias / embedding / residual /
-//                               scale / GroupNorm partial sums -> fp32 and/or fp16 hi/lo)
+//   warpgroup 0   TMA producer  (warp 0: cp.async.bulk.tensor 4-D boxes for A = shifted pixel tiles, 3-D for B)
+//   warpgroups 1, 2  consumers  (rows 0..63 / 64..127 of the 128-row tile: wgmma 64 x BN x 16 fp16, fp32 accumulators in registers;
+//                                in f8 mode the two split-precision correction products are e4m3 wgmmas, 64 x BN x 32, into the
+//                                same accumulators), then the epilogue: accumulators -> shared-memory staging in 64-column chunks ->
+//                                one row per thread: bias / embedding / residual / scale / GroupNorm partial sums -> fp32 and/or
+//                                fp16 hi/lo
 //
-// Pipelines: smem ring (full/empty mbarriers, one or two 64-channel K blocks per stage) between TMA and MMA, and two TMEM accumulator
-// buffers (tmem_full/tmem_empty) between MMA and epilogue so tile i+1 is multiplied while tile i drains.
-// gemm_tc_pair_kernel: the same over a cluster of two CTAs (tcgen05.mma.cta_group::2, M = 256), with row reuse for 3x3 convolutions.
-// Measurement switches (results are garbage, timings are not): DSB_GEMM_DIAG (1 no MMA, 2 no TMA, 4 no epilogue; 8 / 16 no A / B loads,
-// 32 unshifted taps, 64 hot A tile: single-CTA kernel without row reuse only), DSB_GEMM_STAGES, DSB_GEMM_GROUP, DSB_GEMM_RR,
-// DSB_GEMM_EPI_GROUPS, DSB_GEMM_2CTA(_MIN_PAIR_TILES); ds_debug_gemm_trace records the ring timeline of CTA 0.
+// Pipeline: a ring of shared-memory stages (one 64-channel fp16 or 128-channel e4m3 K block of A and B each; full / empty mbarriers)
+// between the producer and the consumers.  The producer runs ahead into the next tile while the consumers drain the current one.
 #include "ops.h"
 #include "ptx.cuh"
 #include <cuda_fp16.h>
@@ -27,8 +24,11 @@
 namespace dsb {
 
 static constexpr int kMaxStages = 8;
-static constexpr int kATileBytes = 128 * 128;   // 128 rows x 64 fp16
-static constexpr int kThreads = 320;           // warp 0: TMA producer, 1: MMA issuer, 2..9: epilogue (two groups of four: even / odd 32-column chunks)
+static constexpr int kATileBytes = 128 * 128;   // 128 rows x 64 fp16 (or 128 e4m3)
+static constexpr int kThreads = 384;           // warpgroup 0: producer (warp 0), 1 and 2: consumers
+static constexpr int kStgPitch = 68;           // floats per row of the epilogue staging buffer (64 columns + 4: conflict-free row reads)
+static constexpr int kStgBytes = 2 * 64 * kStgPitch * 4;
+static constexpr int kSmemLimit = 227 * 1024;
 
 struct alignas(64) GemmKernelParams {
     CUtensorMap tmA, tmA2, tmB;
@@ -65,35 +65,13 @@ struct alignas(64) GemmKernelParams {
     float* st_quads;
     int st_unit;                         // 4 (quads) or 2 (pairs)
     int tap_dh[9], tap_dw[9], tap_cb[9];
-    // CTA-pair variant (gemm_tc_pair_kernel; appended so that the single-CTA kernel's parameter offsets stay put)
-    CUtensorMap tmBh, tmB8h;             // B boxes of BN/2 rows: each CTA of a pair loads half of the N tile
-    int pair;
-    // measurement only (DSB_GEMM_DIAG, profiles/bench_gemm_tiles.py --diag): 1 = no MMAs (operand feed alone), 2 = no TMA loads (MMA issue +
-    // epilogue alone), 4 = no epilogue work (accumulators are released unread).  Results are garbage in every mode but 0.
-    int diag;
-    // debug timeline (ds_debug_gemm_trace, profiles/gemm_timeline.py): CTA 0 stores clock64 per ring stage -- producer after its empty-slot
-    // wait in trace[it], MMA warp after its full-slot wait in trace[trace_cap / 2 + it]; NULL in normal runs
-    unsigned long long* trace;
-    int trace_cap;
-    // K blocks per ring stage (1 or 2): one empty/full barrier round trip, one expect_tx and one tcgen05.commit per `grp` 64-channel blocks.
-    // The role warps' per-stage instruction chains (~500-600 cycles each, r02s/r02t) were longer than the MMAs of a stage whenever BN < 256.
-    int grp;
     int f8_last_steps;                   // e4m3 MMAs (K = 32) of the last 128-channel block of a tap: 2 when only its first 64 channels exist
-                                         // (C = 192, 576: the other two would multiply TMA zero fill with zero-padded weights), else 4
-    int epi_groups;                      // 2 (default): both epilogue warp groups work; 1: group 1 idles (A/B only, DSB_GEMM_EPI_GROUPS)
-    // Row reuse (pair kernel, 3x3 convolutions whose M tile is th = 128 / W whole rows of one image): a ring stage holds ONE (th + 2)-row halo
-    // box of A per (kw, channel block) and the three B blocks of kh = 0, 1, 2; the three taps read the same box through MMA descriptors
-    // offset by kh * W * 128 bytes.  A traffic through L2 and into shared memory: (th + 2) rows per three taps instead of 3 * th.
-    CUtensorMap tmA_rr, tmA8_rr;
-    int rr, rr_halo_bytes, rr_row_bytes;
+                                         // (C = 64, 192, 576: the other two would multiply TMA zero fill with zero-padded weights), else 4
 };
 
 struct SmemCtl {
     uint64_t full[kMaxStages];
     uint64_t empty[kMaxStages];
-    uint64_t tmem_full[2];
-    uint64_t tmem_empty[2];
-    uint32_t tmem_base;
 };
 
 // Sum NV per-lane values over the 32 lanes of a warp with NV-ish shuffles instead of 5*NV: at every butterfly level each lane
@@ -244,8 +222,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKernelParams& p, const 
 
     const long long obase = (long long)zb * p.o_zb + (long long)zh * p.o_zh + grow_in_z * p.ldo + col0;
     // Each thread owns one output row, so a plain 16-byte store per thread writes HALF of 32 different 32-byte sectors per warp
-    // instruction (ncu on the SD ff1 linear: 32 sectors per request, 2x the payload over the crossbar, L2 at 54 % while the tensor pipe
-    // idles at 27 %).  Lanes 2i / 2i+1 swap halves of an 8-float group instead: both then write the two halves of ONE sector of row 2i,
+    // instruction (2x the payload over the crossbar).  Lanes 2i / 2i+1 swap halves of an 8-float group instead: both then write the two halves of ONE sector of row 2i,
     // and of row 2i+1 with the second store -- full sectors only.
     const int odd = threadIdx.x & 1;
     if (p.out_f32) {
@@ -321,54 +298,45 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKernelParams& p, const 
     }
 }
 
-// ------------------------------------------------------------------------------------------ TMA producer: the K loop of one tile
-// r02p/r02q finding (profiles/r02/gemm_feed_diagnosis.txt): with the stage index decoded per iteration (two integer divisions, dynamically
-// indexed parameter loads, a dozen R2UR moves) ONE producer iteration cost ~860 cycles of dependent single-warp latency -- more than the
-// MMAs of a stage (520 e4m3 / 690-780 fp16 cycles) -- so the ring never ran more than one stage ahead and every conv GEMM was bound by the
-// issue rate of its producer warp, not by L2, shared memory or the tensor pipe.  The loop nest below walks (pass, tap, channel block) with
-// running coordinates: no division, one parameter load per tap, everything else loop-invariant.
 struct RingPos {
     int stage;
     uint32_t phase;
 };
 
-// WHICH selects the copies this warp issues (1 = A boxes, 2 = B boxes, 3 = both: the shipped configuration).  Splitting A and B over two
-// producer warps was measured neutral (r02s) once the loop was division-free and stages carry two K blocks, so one warp issues both and
-// the freed warps went to the epilogue.
-template <bool PAIR, int WHICH>
+struct TileCoord {
+    int mt, nt, zb, zh;
+};
+
+__device__ __forceinline__ TileCoord tile_coord(const GemmKernelParams& p, int tile) {
+    const int tiles_per_z = p.m_tiles * p.n_tiles;
+    const int z = tile / tiles_per_z;
+    const int t2 = tile - z * tiles_per_z;
+    TileCoord c;
+    c.mt = t2 / p.n_tiles;
+    c.nt = t2 - c.mt * p.n_tiles;
+    c.zb = z / p.nh;
+    c.zh = z - c.zb * p.nh;
+    return c;
+}
+
+// ------------------------------------------------------------------------------------------ TMA producer: the K loop of one tile
+// Walks (pass, tap, channel block) with running coordinates: no division, one parameter load per tap.  The whole warp runs the loop;
+// one elected lane issues the copies.
 __device__ __forceinline__ void producer_tile(const GemmKernelParams& p, uint8_t* smem, SmemCtl* ctl, RingPos& r, const int block_bytes,
-                                              const uint32_t tx_bytes, const bool arm, const int n_blocks, const int aw0, const int ah0,
-                                              const int an0, const int a_c_off, const int b_k_off, const int b_row, const int b_z, int& trace_n) {
-    const bool ldA = (WHICH & 1) && !(p.diag & (2 | 8)), ldB = (WHICH & 2) && !(p.diag & (2 | 16));
-    const bool tracing = (WHICH & 1) && p.trace && blockIdx.x == 0 && lane_id() == 0;
-    const CUtensorMap* const mB = PAIR ? &p.tmBh : &p.tmB;
-    const CUtensorMap* const mB8 = PAIR ? &p.tmB8h : &p.tmB8;
-    const int grp = p.grp;
-    const int stage_bytes = grp * block_bytes;
-    int sub = 0, left = n_blocks;                           // block inside the current stage; blocks of this tile not yet issued
+                                              const int aw0, const int ah0, const int an0, const int a_c_off, const int b_k_off,
+                                              const int b_row, const int b_z) {
+    const uint32_t tx_bytes = (uint32_t)block_bytes;
     auto load = [&](const CUtensorMap* ma, int ac, int aw, int ah, int an, const CUtensorMap* mb, int bk, int bz) {
-        if (sub == 0) {
-            mbar_wait_warp(&ctl->empty[r.stage], r.phase ^ 1);
-            if (tracing && trace_n < p.trace_cap / 2) p.trace[trace_n++] = clock64();
-        }
-        uint8_t* sa = smem + r.stage * stage_bytes + sub * block_bytes;
+        mbar_wait_warp(&ctl->empty[r.stage], r.phase ^ 1);
+        uint8_t* sa = smem + r.stage * block_bytes;
         uint64_t* full = &ctl->full[r.stage];
         if (elect_one()) {
-            if (arm && sub == 0) mbar_arrive_expect_tx(full, tx_bytes * (uint32_t)min(grp, left));
-            if (PAIR) {
-                if (ldA) tma_load_4d_pair(ma, full, sa, ac, aw, ah, an);
-                if (ldB) tma_load_3d_pair(mb, full, sa + kATileBytes, bk, b_row, bz);
-            } else {
-                if (ldA) tma_load_4d(ma, full, sa, ac, aw, ah, an);
-                if (ldB) tma_load_3d(mb, full, sa + kATileBytes, bk, b_row, bz);
-            }
+            mbar_arrive_expect_tx(full, tx_bytes);
+            tma_load_4d(ma, full, sa, ac, aw, ah, an);
+            tma_load_3d(mb, full, sa + kATileBytes, bk, b_row, bz);
         }
         __syncwarp();
-        --left;
-        if (++sub == grp || left == 0) {
-            sub = 0;
-            if (++r.stage == p.num_stages) { r.stage = 0; r.phase ^= 1; }
-        }
+        if (++r.stage == p.num_stages) { r.stage = 0; r.phase ^= 1; }
     };
     if (p.f8) {
         // e4m3 blocks (128 channels = one 128-byte swizzle row): A_lo8 x W_hi8 over all of K, then A_hi8 x W_lo8
@@ -377,9 +345,9 @@ __device__ __forceinline__ void producer_tile(const GemmKernelParams& p, uint8_t
             int bk = 0;
             for (int tap = 0; tap < p.taps; ++tap) {
                 const int aw = aw0 + p.tap_dw[tap], ah = ah0 + p.tap_dh[tap];
-                for (int cb = 0; cb < p.cpb8; ++cb, bk += 128) load(&p.tmA8, cb * 128, aw, ah, an8, mB8, bk, pass8);
+                for (int cb = 0; cb < p.cpb8; ++cb, bk += 128) load(&p.tmA8, cb * 128, aw, ah, an8, &p.tmB8, bk, pass8);
             }
-            for (int j = 0; j < p.nkb8_aux; ++j, bk += 128) load(&p.tmA2_8, j * 128, aw0, ah0, an8, mB8, bk, pass8);
+            for (int j = 0; j < p.nkb8_aux; ++j, bk += 128) load(&p.tmA2_8, j * 128, aw0, ah0, an8, &p.tmB8, bk, pass8);
         }
     }
     const int npass16 = p.f8 ? 1 : p.npass;                 // fp16 passes: hi x hi (, lo x hi, hi x lo)
@@ -391,96 +359,110 @@ __device__ __forceinline__ void producer_tile(const GemmKernelParams& p, uint8_t
         for (int tap = 0; tap < p.taps; ++tap) {
             const int aw = aw0 + p.tap_dw[tap], ah = ah0 + p.tap_dh[tap];
             const int ac0 = p.tap_cb[tap] + a_c_off;
-            for (int cb = 0; cb < p.cpb; ++cb, bk += 64) load(&p.tmA, ac0 + cb * 64, aw, ah, an, mB, bk, bz);
+            for (int cb = 0; cb < p.cpb; ++cb, bk += 64) load(&p.tmA, ac0 + cb * 64, aw, ah, an, &p.tmB, bk, bz);
         }
-        for (int j = 0; j < p.nkb_aux; ++j, bk += 64) load(&p.tmA2, j * 64, aw0, ah0, an2, mB, bk, bz);
+        for (int j = 0; j < p.nkb_aux; ++j, bk += 64) load(&p.tmA2, j * 64, aw0, ah0, an2, &p.tmB, bk, bz);
     }
 }
 
-// ------------------------------------------------------------------------------------------ MMA issuer: the K loop of one tile
-// Whole warp converged, tcgen05 instructions elected.  One full-barrier wait and one commit per ring stage of p.grp K blocks.
-template <bool PAIR>
+// ------------------------------------------------------------------------------------------ consumer: the K loop of one tile
+// One consumer warpgroup, 64 rows: per ring stage one wgmma group; the stage before it is released once only the newest group is
+// still in flight.
+template <int BN>
 __device__ __forceinline__ void mma_tile(const GemmKernelParams& p, uint8_t* smem, SmemCtl* ctl, RingPos& r, const int block_bytes,
-                                         const int n_iters, const int nkb8x2, const uint32_t idesc, const uint32_t d_tmem,
-                                         uint64_t* tmem_full_bar, int& trace_n) {
-    const int grp = p.grp;
-    const int stage_bytes = grp * block_bytes;
-    const bool tracing = p.trace && blockIdx.x == 0 && lane_id() == 0;
-    // e4m3 blocks of a pass: taps x cpb8 main blocks (the last of each tap may be half empty), then the aux blocks
-    const int nkb8 = nkb8x2 >> 1;
-    int q8 = 0, cb8 = 0;
-    for (int it = 0; it < n_iters; it += grp) {
-        mbar_wait_warp(&ctl->full[r.stage], r.phase);
-        if (tracing && trace_n < p.trace_cap / 2) p.trace[p.trace_cap / 2 + trace_n++] = clock64();
-        tc_fence_after();
-        const uint32_t s0 = smem_u32(smem + r.stage * stage_bytes);
-        const int nb = min(grp, n_iters - it);
-        int steps0 = 4, steps1 = 4;
-        for (int j = 0; j < nb; ++j) {
-            if (it + j < nkb8x2) {
-                if (q8 < p.nkb8_main) {
-                    if (cb8 == p.cpb8 - 1) { if (j == 0) steps0 = p.f8_last_steps; else steps1 = p.f8_last_steps; }
-                    if (++cb8 == p.cpb8) cb8 = 0;
-                }
-                if (++q8 == nkb8) { q8 = 0; cb8 = 0; }
-            }
-        }
-        if (elect_one()) {
-            if (!(p.diag & 1)) {
-                for (int j = 0; j < nb; ++j) {
-                    const uint32_t sa = s0 + j * block_bytes;
-                    const uint64_t da = umma_desc_sw128(sa);
-                    const uint64_t db = umma_desc_sw128(sa + kATileBytes);
-                    const uint32_t acc0 = (it + j) > 0 ? 1u : 0u;
-                    if (it + j < nkb8x2) {
-                        const int ns = j == 0 ? steps0 : steps1;
+                                         const int n_iters, const int nkb8, const int wg, float (&acc)[BN / 2]) {
+    const bool leader = (threadIdx.x & 127) == 0;
+    int prev = -1;
+    for (int it = 0; it < n_iters; ++it) {
+        mbar_wait(&ctl->full[r.stage], r.phase);
+        const uint32_t s0 = smem_u32(smem + r.stage * block_bytes);
+        const uint64_t da = wgmma_desc_sw128(s0 + wg * 64 * 128);
+        const uint64_t db = wgmma_desc_sw128(s0 + kATileBytes);
+        wgmma_fence();
+        if (it < 2 * nkb8) {
+            // e4m3 blocks of a pass: taps x cpb8 main blocks (the last of each tap may be half empty), then the aux blocks
+            const int q8 = it < nkb8 ? it : it - nkb8;
+            const int ns = (q8 < p.nkb8_main && q8 % p.cpb8 == p.cpb8 - 1) ? p.f8_last_steps : 4;
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {       // 32 e4m3 = 32 bytes per MMA: the same +2 descriptor step (16-byte units) as 16 fp16
-                            if (k < ns) {
-                                if (PAIR) umma_f8_pair(d_tmem, da + 2 * k, db + 2 * k, idesc, k > 0 ? 1u : acc0);
-                                else umma_f8(d_tmem, da + 2 * k, db + 2 * k, idesc, k > 0 ? 1u : acc0);
-                            }
-                        }
-                    } else {
+            for (int k = 0; k < 4; ++k)        // 32 e4m3 = 32 bytes per MMA: the same +2 descriptor step (16-byte units) as 16 fp16
+                if (k < ns) wgmma_ss<BN, true>(acc, da + 2 * k, db + 2 * k, (it > 0 || k > 0) ? 1u : 0u);
+        } else {
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            if (PAIR) umma_f16_pair(d_tmem, da + 2 * k, db + 2 * k, idesc, k > 0 ? 1u : acc0);
-                            else umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, k > 0 ? 1u : acc0);
-                        }
-                    }
-                }
-            }
-            if (PAIR) {
-                umma_commit_pair(&ctl->empty[r.stage]);                   // frees this stage in both CTAs
-                if (it + nb >= n_iters) umma_commit_pair(tmem_full_bar);
-            } else {
-                umma_commit(&ctl->empty[r.stage]);
-                if (it + nb >= n_iters) umma_commit(tmem_full_bar);
-            }
+            for (int k = 0; k < 4; ++k) wgmma_ss<BN, false>(acc, da + 2 * k, db + 2 * k, (it > 0 || k > 0) ? 1u : 0u);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_fence_regs(acc);
+        wgmma_wait<1>();
+        if (prev >= 0 && leader) mbar_arrive(&ctl->empty[prev]);
+        prev = r.stage;
         if (++r.stage == p.num_stages) { r.stage = 0; r.phase ^= 1; }
     }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (prev >= 0 && leader) mbar_arrive(&ctl->empty[prev]);
 }
 
+// ------------------------------------------------------------------------------------------ consumer: the epilogue of one tile
+// Accumulator fragment (m64nBN): register g of lane L in warp w holds row 16 w + L / 4 + 8 ((g >> 1) & 1), column 8 (g / 4) + 2 (L % 4)
+// + (g & 1).  Per 64-column chunk the warpgroup stages its 64 x 64 block in shared memory; then warp w takes rows 32 (w & 1) + lane
+// (one row per lane: the layout epilogue_chunk expects, 32-row slabs for the GroupNorm partials) and columns 32 (w >> 1) .. + 32.
+template <int BN>
+__device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, float* stg, const int wg, const TileCoord& tc, const float (&acc)[BN / 2]) {
+    const int lane = threadIdx.x & 31;
+    const int w = (threadIdx.x >> 5) & 3;
+    const int frag_row = 16 * w + (lane >> 2);
+    const int row = 32 * (w & 1) + lane;
+    const long long grow = (long long)tc.mt * 128 + wg * 64 + row;
+    const bool row_ok = grow < p.m_valid;
+#pragma unroll
+    for (int c0 = 0; c0 < BN; c0 += 64) {
+#pragma unroll
+        for (int g = 0; g < 32; g += 2) {
+            const int gi = c0 / 2 + g;
+            if (gi < BN / 2) {
+                const int col = 8 * (g >> 2) + 2 * (lane & 3);
+                const int rr = frag_row + 8 * ((g >> 1) & 1);
+                *reinterpret_cast<float2*>(stg + rr * kStgPitch + col) = make_float2(acc[gi], acc[gi + 1]);
+            }
+        }
+        warpgroup_sync(1 + wg);
+        const int ch = 32 * (w >> 1);
+        const int width = min(32, BN - c0 - ch);
+        const int col0 = tc.nt * BN + c0 + ch;
+        const float* src = stg + row * kStgPitch + ch;
+        if (width >= 32) {
+            float v[32];
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(v + j) = *reinterpret_cast<const float4*>(src + j);
+            if (col0 < p.n_valid) epilogue_chunk<32>(p, v, grow, col0, row_ok, tc.zb, tc.zh, nullptr, false);
+        } else if (width >= 16) {
+            float v[16];
+#pragma unroll
+            for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(v + j) = *reinterpret_cast<const float4*>(src + j);
+            if (col0 < p.n_valid) epilogue_chunk<16>(p, v, grow, col0, row_ok, tc.zb, tc.zh, nullptr, false);
+        }
+        warpgroup_sync(1 + wg);
+    }
+}
+
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmKernelParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // 1024-byte alignment is required by the 128B swizzle; the runtime only guarantees 16.
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int block_bytes = kATileBytes + p.BN * 128;
-    SmemCtl* ctl = reinterpret_cast<SmemCtl*>(smem + p.num_stages * p.grp * block_bytes);
+    const int block_bytes = kATileBytes + BN * 128;
+    float* stg = reinterpret_cast<float*>(smem + p.num_stages * block_bytes);
+    SmemCtl* ctl = reinterpret_cast<SmemCtl*>(smem + p.num_stages * block_bytes + kStgBytes);
 
     const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    int trace_n = 0;
+    const int wg = threadIdx.x >> 7;
     const int nkb_total = p.nkb_main + p.nkb_aux;
     // f8 mode: 2 * nkb8 e4m3 blocks (A_lo8 x W_hi8, then A_hi8 x W_lo8; 128 channels each) followed by the nkb_total fp16 hi x hi blocks
     const int nkb8 = p.f8 ? p.nkb8_main + p.nkb8_aux : 0;
     const int n_iters = p.f8 ? 2 * nkb8 + nkb_total : p.npass * nkb_total;
-    const int tiles_per_z = p.m_tiles * p.n_tiles;
-    const int total_tiles = p.num_z * tiles_per_z;
+    const int total_tiles = p.num_z * p.m_tiles * p.n_tiles;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmA);
         tma_prefetch_desc(&p.tmB);
         if (p.nkb_aux) tma_prefetch_desc(&p.tmA2);
@@ -491,379 +473,53 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
         for (int s = 0; s < p.num_stages; ++s) {
             mbar_init(&ctl->full[s], 1);
-            mbar_init(&ctl->empty[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&ctl->tmem_full[a], 1);
-            mbar_init(&ctl->tmem_empty[a], 8);                            // the eight epilogue warps
+            mbar_init(&ctl->empty[s], 2);                                 // one arrival per consumer warpgroup
         }
         fence_barrier_init();
-    } else if (warp == 1) {
-        tmem_alloc(&ctl->tmem_base, 512);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = ctl->tmem_base;
 
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer (whole warp converged; the copies elected)
-        {
+    if (wg == 0) {
+        // ------------------------------------------------------------------ TMA producer (warp 0, converged; the copies elected)
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 0) {
             RingPos ring{0, 0u};
-            const uint32_t tx_bytes = (p.diag & 2) ? 0u : (uint32_t)(((p.diag & 8) ? 0 : kATileBytes) + ((p.diag & 16) ? 0 : p.BN * 128));
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                const int z = tile / tiles_per_z;
-                const int t2 = tile - z * tiles_per_z;
-                const int mt = t2 / p.n_tiles;
-                const int nt = t2 - mt * p.n_tiles;
-                const int zb = z / p.nh, zh = z - zb * p.nh;
+                const TileCoord tc = tile_coord(p, tile);
                 int aw0, ah0, an0;
                 if (p.a_mode == 0) {
+                    // 128 consecutive NHWC pixels: whole image rows (W <= 128) or a 128-pixel segment of one row (W a multiple of 128)
                     const int HW = p.conv_H * p.conv_W;
-                    const int p0 = (p.diag & 64) ? 0 : mt * 128;
+                    const int p0 = tc.mt * 128;
                     an0 = p0 / HW;
-                    ah0 = (p0 - an0 * HW) / p.conv_W;
-                    aw0 = 0;
+                    const int rem = p0 - an0 * HW;
+                    ah0 = rem / p.conv_W;
+                    aw0 = rem - ah0 * p.conv_W;
                 } else {
-                    aw0 = mt * 128;
+                    aw0 = tc.mt * 128;
                     ah0 = 0;
-                    an0 = zb * p.a_n_per_zb + zh * p.a_n_per_zh;
+                    an0 = tc.zb * p.a_n_per_zb + tc.zh * p.a_n_per_zh;
                 }
-                const int a_c_off = zh * p.a_c_per_zh;
-                const int b_k_off = p.b_k0 + zh * p.b_k_per_zh;
-                const int b_row = nt * p.BN + zh * p.b_row_per_zh;
-                const int b_z = zb * p.b_z_per_zb + zh * p.b_z_per_zh;
-                producer_tile<false, 3>(p, smem, ctl, ring, block_bytes, tx_bytes, true, n_iters, aw0, ah0, an0, a_c_off, b_k_off, b_row, b_z, trace_n);
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (whole warp converged; tcgen05 instructions elected)
-        {
-            const uint32_t idesc = umma_idesc_f16((uint32_t)p.BN);
-            RingPos ring{0, 0u};
-            int iter = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-                const int acc = iter & 1;
-                const uint32_t acc_phase = (iter >> 1) & 1;
-                mbar_wait_warp(&ctl->tmem_empty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                mma_tile<false>(p, smem, ctl, ring, block_bytes, n_iters, 2 * nkb8, idesc, tmem_base + acc * 256, &ctl->tmem_full[acc], trace_n);
+                const int a_c_off = tc.zh * p.a_c_per_zh;
+                const int b_k_off = p.b_k0 + tc.zh * p.b_k_per_zh;
+                const int b_row = tc.nt * BN + tc.zh * p.b_row_per_zh;
+                const int b_z = tc.zb * p.b_z_per_zb + tc.zh * p.b_z_per_zh;
+                producer_tile(p, smem, ctl, ring, block_bytes, aw0, ah0, an0, a_c_off, b_k_off, b_row, b_z);
             }
         }
     } else {
-        // ------------------------------------------------------------------ epilogue (warps 2..9: two groups of four)
-        const int quad = warp & 3;   // TMEM lane quadrant this warp may access
-        const int eg = (warp - 2) >> 2;
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-            const int z = tile / tiles_per_z;
-            const int t2 = tile - z * tiles_per_z;
-            const int mt = t2 / p.n_tiles;
-            const int nt = t2 - mt * p.n_tiles;
-            const int zb = z / p.nh, zh = z - zb * p.nh;
-            const int acc = iter & 1;
-            const uint32_t acc_phase = (iter >> 1) & 1;
-            mbar_wait(&ctl->tmem_full[acc], acc_phase);
-            tc_fence_after();
-            const int row = quad * 32 + lane;
-            const long long grow = (long long)mt * 128 + row;
-            const bool row_ok = grow < p.m_valid;
-            const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * 256;
-            // residual rows are prefetched one chunk ahead (registers) so their HBM latency overlaps the previous chunk's work
-            const float* res_row = p.residual ? p.residual + (row_ok ? grow : 0) * p.ldr + (long long)nt * p.BN : nullptr;
-            float4 res_next[8];
-            auto prefetch = [&](int cc) {
-                if (res_row && (long long)nt * p.BN + cc + 32 <= p.n_valid) {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) res_next[q] = *reinterpret_cast<const float4*>(res_row + cc + 4 * q);
-                }
-            };
-            // epilogue group eg takes the 32-column chunks eg, eg + 2, ... (and the 16-column tail if it is its turn)
-            const int cstep = 32 * p.epi_groups;
-            if (!(p.diag & 4) && eg < p.epi_groups && eg * 32 + 32 <= p.BN) prefetch(eg * 32);
-            int c = ((p.diag & 4) || eg >= p.epi_groups) ? p.BN : eg * 32;
-            for (; c + 32 <= p.BN; c += cstep) {
-                float4 res_cur[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) res_cur[q] = res_next[q];
-                const int col0 = nt * p.BN + c;
-                const bool in_regs = res_row && (col0 + 32 <= p.n_valid);
-                if (c + cstep + 32 <= p.BN) prefetch(c + cstep);
-                uint32_t v[32];
-                DSB_TMEM_LD_32(t_row + c, v);
-                tmem_ld_wait();
-                if (col0 < p.n_valid)
-                    epilogue_chunk<32>(p, reinterpret_cast<const float*>(v), grow, col0, row_ok, zb, zh, res_cur, in_regs);
-            }
-            if (c < p.BN && c + 32 > p.BN && !(p.diag & 4)) {
-                uint32_t v[16];
-                DSB_TMEM_LD_16(t_row + c, v);
-                tmem_ld_wait();
-                const int col0 = nt * p.BN + c;
-                if (col0 < p.n_valid)
-                    epilogue_chunk<16>(p, reinterpret_cast<const float*>(v), grow, col0, row_ok, zb, zh, nullptr, false);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&ctl->tmem_empty[acc]);
+        // ------------------------------------------------------------------ consumers (warpgroups 1, 2: rows 0..63 / 64..127)
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        const int cw = wg - 1;
+        float* my_stg = stg + cw * 64 * kStgPitch;
+        RingPos ring{0, 0u};
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const TileCoord tc = tile_coord(p, tile);
+            float acc[BN / 2];
+            mma_tile<BN>(p, smem, ctl, ring, block_bytes, n_iters, nkb8, cw, acc);
+            epilogue_tile<BN>(p, my_stg, cw, tc, acc);
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
-}
-
-// ------------------------------------------------------------------------------------------ row-reuse K loops (pair kernel only)
-// Stage sequence of a tile, identical in the producers and in the MMA warp:
-//   f8:   for pass8 in {A_lo8 x W_hi8, A_hi8 x W_lo8}: for kw: for channel block (128): MAIN;  then the aux (1x1 skip) blocks
-//   fp16: for pass:                                      for kw: for channel block (64):  MAIN;  then the aux blocks
-// MAIN = [A halo box][B kh=0][B kh=1][B kh=2], aux = [A 128-pixel tile][B].  Weights stay packed K = (kh, kw, cin).
-template <int WHICH>
-__device__ __forceinline__ void producer_tile_rr(const GemmKernelParams& p, uint8_t* smem, SmemCtl* ctl, RingPos& r, const int stage_bytes,
-                                                 const int hb, const bool arm, const int aw0, const int ah0, const int an0, const int b_row,
-                                                 int& trace_n) {
-    const bool tracing = (WHICH & 1) && p.trace && blockIdx.x == 0 && lane_id() == 0;
-    const uint32_t tx_main = 2u * (uint32_t)(((WHICH & 1) ? p.rr_halo_bytes : 0) + ((WHICH & 2) ? 3 * hb : 0));   // both CTAs' bytes land on the leader's barrier
-    const uint32_t tx_aux = 2u * (uint32_t)(((WHICH & 1) ? kATileBytes : 0) + ((WHICH & 2) ? hb : 0));
-    // one stage: wait for the slot, arm, issue this warp's copies
-    auto stage = [&](bool main, const CUtensorMap* ma, int ac, int aw, int ah, int an, const CUtensorMap* mb, int bk0, int bk_step, int bz) {
-        mbar_wait_warp(&ctl->empty[r.stage], r.phase ^ 1);
-        if (tracing && trace_n < p.trace_cap / 2) p.trace[trace_n++] = clock64();
-        uint8_t* sa = smem + r.stage * stage_bytes;
-        uint64_t* full = &ctl->full[r.stage];
-        if (elect_one()) {
-            if (arm) mbar_arrive_expect_tx(full, main ? tx_main : tx_aux);
-            if (WHICH & 1) tma_load_4d_pair(ma, full, sa, ac, aw, ah, an);
-            if (WHICH & 2) {
-                uint8_t* sb = sa + p.rr_halo_bytes;
-                tma_load_3d_pair(mb, full, sb, bk0, b_row, bz);
-                if (main) {
-                    tma_load_3d_pair(mb, full, sb + hb, bk0 + bk_step, b_row, bz);
-                    tma_load_3d_pair(mb, full, sb + 2 * hb, bk0 + 2 * bk_step, b_row, bz);
-                }
-            }
-        }
-        __syncwarp();
-        if (++r.stage == p.num_stages) { r.stage = 0; r.phase ^= 1; }
-    };
-    if (p.f8) {
-        const int kh_step = 3 * p.cpb8 * 128;                       // K distance between kh and kh + 1 (bytes = e4m3 elements)
-        for (int pass8 = 0; pass8 < 2; ++pass8) {
-            const int an8 = an0 + pass8 * p.a8_plane_n;
-            for (int kw = 0; kw < 3; ++kw)
-                for (int cb = 0; cb < p.cpb8; ++cb)
-                    stage(true, &p.tmA8_rr, cb * 128, aw0 + kw - 1, ah0 - 1, an8, &p.tmB8h, (kw * p.cpb8 + cb) * 128, kh_step, pass8);
-            for (int j = 0; j < p.nkb8_aux; ++j)
-                stage(false, &p.tmA2_8, j * 128, aw0, ah0, an8, &p.tmB8h, (9 * p.cpb8 + j) * 128, 0, pass8);
-        }
-    }
-    const int npass16 = p.f8 ? 1 : p.npass;
-    const int kh_step = 3 * p.cpb * 64;
-    for (int pass = 0; pass < npass16; ++pass) {
-        const int an = an0 + (pass == 1 ? p.a_plane_n : 0);
-        const int an2 = an0 + (pass == 1 ? p.a2_plane_n : 0);
-        const int bz = pass == 2 ? p.b_plane_batch : 0;
-        for (int kw = 0; kw < 3; ++kw)
-            for (int cb = 0; cb < p.cpb; ++cb)
-                stage(true, &p.tmA_rr, cb * 64, aw0 + kw - 1, ah0 - 1, an, &p.tmBh, (kw * p.cpb + cb) * 64, kh_step, bz);
-        for (int j = 0; j < p.nkb_aux; ++j)
-            stage(false, &p.tmA2, j * 64, aw0, ah0, an2, &p.tmBh, (9 * p.cpb + j) * 64, 0, bz);
-    }
-}
-
-__device__ __forceinline__ void mma_tile_rr(const GemmKernelParams& p, uint8_t* smem, SmemCtl* ctl, RingPos& r, const int stage_bytes,
-                                            const int hb, const uint32_t idesc, const uint32_t d_tmem, uint64_t* tmem_full_bar, int& trace_n) {
-    const bool tracing = p.trace && blockIdx.x == 0 && lane_id() == 0;
-    const int main8 = p.f8 ? 3 * p.cpb8 : 0, aux8 = p.f8 ? p.nkb8_aux : 0;
-    const int npass16 = p.f8 ? 1 : p.npass;
-    const int main16 = 3 * p.cpb, aux16 = p.nkb_aux;
-    const int n_f8 = 2 * (main8 + aux8);
-    const int n_stages = n_f8 + npass16 * (main16 + aux16);
-    int q = 0;                                   // stage index inside the current pass
-    int cb8 = 0;
-    int per_pass = main8 + aux8, n_main = main8;
-    for (int st = 0; st < n_stages; ++st) {
-        if (st == n_f8) { q = 0; per_pass = main16 + aux16; n_main = main16; }
-        const bool f8 = st < n_f8;
-        const bool main = q < n_main;
-        mbar_wait_warp(&ctl->full[r.stage], r.phase);
-        if (tracing && trace_n < p.trace_cap / 2) p.trace[p.trace_cap / 2 + trace_n++] = clock64();
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + r.stage * stage_bytes);
-        const uint32_t sb = sa + p.rr_halo_bytes;
-        int ns = 4;                              // main stages of a pass run (kw, channel block): the last channel block may be half empty
-        if (f8 && main) {
-            if (cb8 == p.cpb8 - 1) ns = p.f8_last_steps;
-            if (++cb8 == p.cpb8) cb8 = 0;
-        }
-        if (elect_one()) {
-            if (!(p.diag & 1)) {
-                const int nkh = main ? 3 : 1;
-                for (int kh = 0; kh < nkh; ++kh) {
-                    const uint64_t da = umma_desc_sw128(sa + kh * p.rr_row_bytes);
-                    const uint64_t db = umma_desc_sw128(sb + kh * hb);
-                    const uint32_t acc0 = (st > 0 || kh > 0) ? 1u : 0u;
-                    if (f8) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            if (k < ns) umma_f8_pair(d_tmem, da + 2 * k, db + 2 * k, idesc, k > 0 ? 1u : acc0);
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) umma_f16_pair(d_tmem, da + 2 * k, db + 2 * k, idesc, k > 0 ? 1u : acc0);
-                    }
-                }
-            }
-            umma_commit_pair(&ctl->empty[r.stage]);
-            if (st == n_stages - 1) umma_commit_pair(tmem_full_bar);
-        }
-        __syncwarp();
-        if (++r.stage == p.num_stages) { r.stage = 0; r.phase ^= 1; }
-        if (++q == per_pass) q = 0;
-    }
-}
-
-// ------------------------------------------------------------------------------------------ CTA-pair variant (large convolutions; DSB_GEMM_2CTA=0 disables)
-// Same roles and pipelines over a cluster of two CTAs (one TPC): the pair owns 256 output rows (M tiles 2*pm + rank) x BN columns; each
-// CTA loads its own 128-row A tile and HALF of the B tile, the leader (rank 0) issues tcgen05.mma.cta_group::2 (M = 256) whose
-// accumulator halves land in the two CTAs' TMEM, and each CTA's epilogue warps drain their own half.  Per 64-channel K block a pair pulls
-// 2 x 16 KB (A) + BN x 128 B (B, once) through L2 instead of 2 x (16 KB + BN x 128 B): -33 % at BN = 256, and the 32 KB stages give a
-// 7-deep ring instead of 4.  (The single-CTA kernel is L2-feed bound at ~14 TB/s, profiles/r01c.)
-// Barriers: full[s] lives in the leader (armed with both CTAs' bytes; both CTAs' TMA complete_tx on it), empty[s] and tmem_full[a] are
-// signalled in both CTAs by multicast commits, tmem_empty[a] in the leader collects the eight epilogue warps of the pair.
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1) gemm_tc_pair_kernel(const __grid_constant__ GemmKernelParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int half_bn = p.BN >> 1;
-    const int block_bytes = kATileBytes + half_bn * 128;
-    const int rr_stage_bytes = p.rr_halo_bytes + 3 * half_bn * 128;
-    SmemCtl* ctl = reinterpret_cast<SmemCtl*>(smem + p.num_stages * (p.rr ? rr_stage_bytes : p.grp * block_bytes));
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    int trace_n = 0;
-    const int rank = (int)cluster_ctarank();
-    const int nkb_total = p.nkb_main + p.nkb_aux;
-    const int nkb8 = p.f8 ? p.nkb8_main + p.nkb8_aux : 0;
-    const int n_iters = p.f8 ? 2 * nkb8 + nkb_total : p.npass * nkb_total;
-    const int pair_m_tiles = (p.m_tiles + 1) >> 1;
-    const int total_tiles = pair_m_tiles * p.n_tiles;                     // num_z == 1 (checked on the host)
-    const int first = (int)cluster_id_x(), step = (int)cluster_count_x();
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(p.rr ? &p.tmA_rr : &p.tmA);
-        tma_prefetch_desc(&p.tmBh);
-        if (p.nkb_aux) tma_prefetch_desc(&p.tmA2);
-        if (p.f8) {
-            tma_prefetch_desc(&p.tmA8);
-            tma_prefetch_desc(&p.tmB8h);
-            if (p.nkb8_aux) tma_prefetch_desc(&p.tmA2_8);
-        }
-        for (int s = 0; s < p.num_stages; ++s) {
-            mbar_init(&ctl->full[s], 1);                                  // the leader's producer warp arms both CTAs' bytes
-            mbar_init(&ctl->empty[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&ctl->tmem_full[a], 1);
-            mbar_init(&ctl->tmem_empty[a], 16);                           // 8 epilogue warps of each CTA (used in the leader only)
-        }
-        fence_barrier_init();
-    } else if (warp == 1) {
-        tmem_alloc_pair(&ctl->tmem_base, 512);
-    }
-    tc_fence_before();
-    cluster_sync_all();                                                   // both CTAs' barriers and TMEM exist before any remote use
-    tc_fence_after();
-    const uint32_t tmem_base = ctl->tmem_base;
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer (both CTAs; warp converged, copies elected)
-        {
-            RingPos ring{0, 0u};
-            // the leader's full barrier collects both CTAs' bytes
-            const uint32_t tx_bytes = (p.diag & 2) ? 0u : 2u * (uint32_t)(((p.diag & 8) ? 0 : kATileBytes) + ((p.diag & 16) ? 0 : half_bn * 128));
-            for (int tile = first; tile < total_tiles; tile += step) {
-                const int pm = tile / p.n_tiles;
-                const int nt = tile - pm * p.n_tiles;
-                const int mt = 2 * pm + rank;                             // may be one past the last tile: TMA zero-fills, the epilogue masks
-                // 128 consecutive NHWC pixels: whole image rows (W <= 128, box (64, W, 128/W.., ..)) or a 128-pixel segment of one row
-                // (W a multiple of 128 > 128, box (64, 128, 1, 1): the first-stage decoder's 256- and 512-wide layers)
-                const int HW = p.conv_H * p.conv_W;
-                const int p0 = (p.diag & 64) ? rank * 128 : mt * 128;
-                const int an0 = p0 / HW;
-                const int rem = p0 - an0 * HW;
-                const int ah0 = rem / p.conv_W;
-                const int aw0 = rem - ah0 * p.conv_W;
-                const int b_row = nt * p.BN + rank * half_bn;
-                if (p.rr) producer_tile_rr<3>(p, smem, ctl, ring, rr_stage_bytes, half_bn * 128, rank == 0, aw0, ah0, an0, b_row, trace_n);
-                else producer_tile<true, 3>(p, smem, ctl, ring, block_bytes, tx_bytes, rank == 0, n_iters, aw0, ah0, an0, 0, 0, b_row, 0, trace_n);
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (leader CTA only; warp converged, tcgen05 elected)
-        if (rank == 0) {
-            const uint32_t idesc = umma_idesc_pair((uint32_t)p.BN);
-            RingPos ring{0, 0u};
-            int iter = 0;
-            for (int tile = first; tile < total_tiles; tile += step, ++iter) {
-                const int acc = iter & 1;
-                const uint32_t acc_phase = (iter >> 1) & 1;
-                mbar_wait_warp(&ctl->tmem_empty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                if (p.rr) mma_tile_rr(p, smem, ctl, ring, rr_stage_bytes, half_bn * 128, idesc, tmem_base + acc * 256, &ctl->tmem_full[acc], trace_n);
-                else mma_tile<true>(p, smem, ctl, ring, block_bytes, n_iters, 2 * nkb8, idesc, tmem_base + acc * 256, &ctl->tmem_full[acc], trace_n);
-            }
-        }
-    } else {
-        // ------------------------------------------------------------------ epilogue (warps 2..9 of both CTAs, own 128 rows each)
-        const int quad = warp & 3;
-        const int eg = (warp - 2) >> 2;
-        int iter = 0;
-        for (int tile = first; tile < total_tiles; tile += step, ++iter) {
-            const int pm = tile / p.n_tiles;
-            const int nt = tile - pm * p.n_tiles;
-            const int mt = 2 * pm + rank;
-            const int acc = iter & 1;
-            const uint32_t acc_phase = (iter >> 1) & 1;
-            mbar_wait(&ctl->tmem_full[acc], acc_phase);
-            tc_fence_after();
-            const int row = quad * 32 + lane;
-            const long long grow = (long long)mt * 128 + row;
-            const bool row_ok = grow < p.m_valid;
-            const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * 256;
-            const float* res_row = p.residual ? p.residual + (row_ok ? grow : 0) * p.ldr + (long long)nt * p.BN : nullptr;
-            float4 res_next[8];
-            auto prefetch = [&](int cc) {
-                if (res_row && (long long)nt * p.BN + cc + 32 <= p.n_valid) {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) res_next[q] = *reinterpret_cast<const float4*>(res_row + cc + 4 * q);
-                }
-            };
-            const int cstep = 32 * p.epi_groups;
-            if (!(p.diag & 4) && eg < p.epi_groups && eg * 32 + 32 <= p.BN) prefetch(eg * 32);
-            int c = ((p.diag & 4) || eg >= p.epi_groups) ? p.BN : eg * 32;
-            for (; c + 32 <= p.BN; c += cstep) {
-                float4 res_cur[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) res_cur[q] = res_next[q];
-                const int col0 = nt * p.BN + c;
-                const bool in_regs = res_row && (col0 + 32 <= p.n_valid);
-                if (c + cstep + 32 <= p.BN) prefetch(c + cstep);
-                uint32_t v[32];
-                DSB_TMEM_LD_32(t_row + c, v);
-                tmem_ld_wait();
-                if (col0 < p.n_valid)
-                    epilogue_chunk<32>(p, reinterpret_cast<const float*>(v), grow, col0, row_ok, 0, 0, res_cur, in_regs);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_leader(&ctl->tmem_empty[acc]);
-        }
-    }
-
-    tc_fence_before();
-    cluster_sync_all();                      // the leader's MMAs read the peer's shared memory; neither CTA may exit before both are done
-    if (warp == 1) tmem_dealloc_pair(tmem_base, 512);
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -902,14 +558,6 @@ static int encode_map_typed(CUtensorMap* m, const void* ptr, int rank, const int
         return -2;
     }
     return 0;
-}
-
-static unsigned long long* g_trace_buf = nullptr;
-static int g_trace_cap = 0;
-
-static bool all_tap_cb_zero(const ds_gemm_desc* d) {
-    for (int t = 0; t < 9; ++t) if (d->tap_cb[t]) return false;
-    return true;
 }
 
 // fp16 tensors (also used by attention.cu)
@@ -962,8 +610,7 @@ int gemm_build(const ds_gemm_desc* d, GemmKernelParams* kp) {
         const char* a8 = static_cast<const char*>(d->a_ptr) + Bn * Hd * Wd * C * 2;
         if (encode_map_typed(&kp->tmA8, a8, 4, dims8, st8, box8, true)) return -17;
         kp->f8 = 1;
-        static const int half_env = [] { const char* e = getenv("DSB_GEMM_F8_HALF"); return e ? atoi(e) : 1; }();
-        kp->f8_last_steps = (half_env && (d->cpb & 1)) ? 2 : 4;
+        kp->f8_last_steps = (d->cpb & 1) ? 2 : 4;
         kp->a8_plane_n = (int)Bn;
         kp->cpb8 = (d->cpb + 1) / 2;
         kp->nkb8_main = d->taps * kp->cpb8;
@@ -985,134 +632,67 @@ int gemm_build(const ds_gemm_desc* d, GemmKernelParams* kp) {
         if (encode_map_typed(&kp->tmB8, b8, 3, bd8, bs8, bbox8, true)) return -19;
     }
     for (int t = 0; t < 9; ++t) { kp->tap_dh[t] = d->tap_dh[t]; kp->tap_dw[t] = d->tap_dw[t]; kp->tap_cb[t] = d->tap_cb[t]; }
-    { const char* e = getenv("DSB_GEMM_DIAG"); kp->diag = e ? atoi(e) : 0; }
-    { const char* e = getenv("DSB_GEMM_EPI_GROUPS"); kp->epi_groups = (e && atoi(e) == 1) ? 1 : 2; }
-    kp->trace = g_trace_buf; kp->trace_cap = g_trace_cap;
-    if (kp->diag & 32) for (int t = 0; t < 9; ++t) { kp->tap_dh[t] = 0; kp->tap_dw[t] = 0; }      // every tap reads the unshifted box
     if (d->taps != 1 && d->taps != 9) return -15;
-    // image rows wider than one M tile are only handled by the pair kernel's tile -> (w, h, n) mapping
-    if (d->a_mode == 0 && d->conv_W > 128 && !((d->f8 & 2) && d->BN % 32 == 0 && d->num_z == 1 && d->conv_W % 128 == 0)) return -13;
+    // image rows wider than one M tile: the tile is a 128-pixel segment of one row
+    if (d->a_mode == 0 && d->conv_W > 128 && (d->conv_W % 128 != 0 || d->a_box[1] != 128)) return -13;
     // fused statistics: whole 32-row slabs (row validity is then warp-uniform), whole channel quads, one z slice, fp32 output
     if (d->st_quads && (d->num_z != 1 || d->m_valid % 32 != 0 || d->n_valid % (d->st_unit == 2 ? 2 : 4) != 0 || d->edm_out != 0)) return -14;
-    int stage_bytes = kATileBytes + d->BN * 128;
-    // CTA-pair variant (opt-in): convolution GEMMs with at least two full waves of row pairs and an N tile that splits into two
-    // whole 32-row halves; everything else keeps the single-CTA kernel
-    // default ON since round 2: bit-identical to the single-CTA kernel (tests/test_gpu_kernels.py::test_conv_pair_kernel) and +2.8 % images/s on the
-    // power-capped sustained bench (profiles/r02b: 513.2 vs 499.0): a third fewer operand bytes through L2 / shared memory per FLOP.
-    static const int pair_env = [] { const char* e = getenv("DSB_GEMM_2CTA"); return e ? atoi(e) : 1; }();
-    const bool pair_forced = (d->f8 & 2) != 0;          // bit 1 of ds_gemm_desc.f8: request the pair kernel for this launch (tests, A/B)
-    // since the producer rewrite (r02r) the pair kernel runs at the MMA instruction bound (600 cycles per stage) while the single-CTA kernel
-    // is shared-memory-port bound (770): the pair wins 12-16 % on every shape that still gives each SM pair a tile
-    static const int pair_min_tiles = [] { const char* e = getenv("DSB_GEMM_2CTA_MIN_PAIR_TILES"); return e ? atoi(e) : 74; }();
-    const bool pair_auto = pair_env && ((d->m_tiles + 1) / 2) * d->n_tiles >= pair_min_tiles && d->BN >= 32;
-    const bool diag_single_only = (kp->diag & (8 | 16)) != 0;      // the A-only / B-only feed measurements exist for the single-CTA kernel only
-    if ((pair_forced || pair_auto) && !diag_single_only && d->a_mode == 0 && d->num_z == 1 && d->b_k0 == 0 && d->BN % 32 == 0 &&
-        all_tap_cb_zero(d)) {
-        int32_t hbox[3] = {64, d->BN / 2, 1};
-        if (encode_map(&kp->tmBh, d->b_ptr, 3, d->b_dims, d->b_strides, hbox)) return -30;
-        if (d->f8 & 1) {
-            const int64_t ktot8 = (int64_t)(kp->nkb8_main + kp->nkb8_aux) * 128;
-            const int64_t rows = d->b_dims[1];
-            const int64_t bd8[3] = {ktot8, rows, 2};
-            const int64_t bs8[2] = {ktot8, rows * ktot8};
-            const int32_t hbox8[3] = {128, d->BN / 2, 1};
-            const char* b8 = static_cast<const char*>(d->b_ptr) + rows * d->b_dims[0] * 2;
-            if (encode_map_typed(&kp->tmB8h, b8, 3, bd8, bs8, hbox8, true)) return -31;
-        }
-        kp->pair = 1;
-        stage_bytes = kATileBytes + (d->BN / 2) * 128;
-        // row reuse: plain 3x3 taps, the M tile = th >= 2 whole rows of one image (W <= 64), at least three stages of halo + 3 B blocks
-        static const int rr_env = [] { const char* e = getenv("DSB_GEMM_RR"); return e ? atoi(e) : 1; }();
-        const int Wd = (int)d->a_dims[1], Hd = (int)d->a_dims[2];
-        bool std_taps = d->taps == 9;
-        for (int t = 0; t < 9 && std_taps; ++t) std_taps = d->tap_dh[t] == t / 3 - 1 && d->tap_dw[t] == t % 3 - 1;
-        const int th = Wd > 0 ? 128 / Wd : 0;
-        const int halo = (th + 2) * Wd * 128;
-        const int rr_stage = halo + 3 * (d->BN / 2) * 128;
-        if (rr_env && !(kp->diag & (2 | 32 | 64)) && std_taps && Wd <= 64 && th >= 2 && th * Wd == 128 && Hd % th == 0 && d->a_box[1] == Wd && d->a_box[2] == th && d->a_box[3] == 1 &&
-            d->conv_W == Wd && d->conv_H == Hd && (227 * 1024 - 2048) / rr_stage >= 3) {
-            const int32_t box_rr[4] = {64, Wd, th + 2, 1};
-            if (encode_map(&kp->tmA_rr, d->a_ptr, 4, d->a_dims, d->a_strides, box_rr)) return -32;
-            if (d->f8 & 1) {
-                const int64_t C = d->a_dims[0], Bn = d->a_plane_n;
-                const int32_t box8_rr[4] = {128, Wd, th + 2, 1};
-                const int64_t dims8[4] = {C, Wd, Hd, 2 * Bn};
-                const int64_t st8[3] = {C, (int64_t)Wd * C, (int64_t)Hd * Wd * C};
-                const char* a8 = static_cast<const char*>(d->a_ptr) + Bn * Hd * Wd * C * 2;
-                if (encode_map_typed(&kp->tmA8_rr, a8, 4, dims8, st8, box8_rr, true)) return -33;
-            }
-            kp->rr = 1;
-            kp->rr_halo_bytes = halo;
-            kp->rr_row_bytes = Wd * 128;
-        }
-    }
-    // two K blocks per ring stage when at least three (pair) / four (single) such stages still fit
-    static const int grp_env = [] { const char* e = getenv("DSB_GEMM_GROUP"); return e ? atoi(e) : 2; }();
-    kp->grp = 1;
-    if (kp->rr) stage_bytes = kp->rr_halo_bytes + 3 * (d->BN / 2) * 128;
-    else if (grp_env == 2 && (227 * 1024 - 2048) / (2 * stage_bytes) >= (kp->pair ? 3 : 4)) { kp->grp = 2; stage_bytes *= 2; }
-    int ns = (227 * 1024 - 2048) / stage_bytes;
+    const int stage_bytes = kATileBytes + d->BN * 128;
+    int ns = (kSmemLimit - 1024 - kStgBytes - (int)sizeof(SmemCtl)) / stage_bytes;
     if (ns > kMaxStages) ns = kMaxStages;
-    { const char* e = getenv("DSB_GEMM_STAGES"); if (e && atoi(e) >= 2 && atoi(e) < ns) ns = atoi(e); }      // measurement only
     kp->num_stages = ns;
     return 0;
 }
-
-void gemm_set_trace(unsigned long long* buf, int cap) { g_trace_buf = buf; g_trace_cap = cap; }
 
 size_t gemm_params_size() { return sizeof(GemmKernelParams); }
 void gemm_patch_edm(GemmKernelParams* kp, const float* x, float* D) { kp->edm_x = x; kp->edm_D = D; }
 
 // cudaFuncSetAttribute is per device: one process may drive several GPUs (tests, notebooks), so the opt-in shared-memory size is set once per
-// (device, kernel) and the SM count is kept per device.
+// (device, N tile) and the SM count is kept per device.
 static int g_num_sms[64] = {};
-static bool g_attr_set[64] = {};
-static bool g_pair_attr_set[64] = {};
+static bool g_attr_set[64][17] = {};
 
-static int current_device_slot() {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    return (dev < 0 || dev >= 64) ? 0 : dev;
-}
-
-static int gemm_run_pair(const GemmKernelParams* kp, cudaStream_t stream, int slot) {
-    if (!g_pair_attr_set[slot]) {
-        if (cudaFuncSetAttribute(gemm_tc_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) return -22;
-        g_pair_attr_set[slot] = true;
+template <int BN>
+static int gemm_launch(const GemmKernelParams* kp, cudaStream_t stream, int slot) {
+    if (!g_attr_set[slot][BN / 16]) {
+        if (cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess) return -20;
+        g_attr_set[slot][BN / 16] = true;
     }
-    const int stage_bytes = kp->rr ? kp->rr_halo_bytes + 3 * (kp->BN / 2) * 128 : kp->grp * (kATileBytes + (kp->BN / 2) * 128);
-    const size_t smem = (size_t)kp->num_stages * stage_bytes + sizeof(SmemCtl) + 1024;
-    const int tiles = ((kp->m_tiles + 1) / 2) * kp->n_tiles;
-    int clusters = g_num_sms[slot] / 2;
-    if (tiles < clusters) clusters = tiles;
-    if (clusters <= 0) return 0;
-    gemm_tc_pair_kernel<<<2 * clusters, kThreads, smem, stream>>>(*kp);       // cluster shape (2,1,1) is part of the kernel (__cluster_dims__)
-    return cudaGetLastError() == cudaSuccess ? 0 : -23;
-}
-
-int gemm_run(const GemmKernelParams* kp, cudaStream_t stream) {
-    const int slot = current_device_slot();
-    if (!g_attr_set[slot]) {
-        cudaDeviceGetAttribute(&g_num_sms[slot], cudaDevAttrMultiProcessorCount, slot);
-        if (cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) return -20;
-        g_attr_set[slot] = true;
-    }
-    if (kp->pair) return gemm_run_pair(kp, stream, slot);
-    const int stage_bytes = kp->grp * (kATileBytes + kp->BN * 128);
-    const size_t smem = (size_t)kp->num_stages * stage_bytes + sizeof(SmemCtl) + 1024;
+    const size_t smem = (size_t)kp->num_stages * (kATileBytes + BN * 128) + kStgBytes + sizeof(SmemCtl) + 1024;
     const int tiles = kp->num_z * kp->m_tiles * kp->n_tiles;
     const int grid = tiles < g_num_sms[slot] ? tiles : g_num_sms[slot];
     if (grid <= 0) return 0;
-    gemm_tc_kernel<<<grid, kThreads, smem, stream>>>(*kp);
+    gemm_tc_kernel<BN><<<grid, kThreads, smem, stream>>>(*kp);
     return cudaGetLastError() == cudaSuccess ? 0 : -21;
 }
 
-}  // namespace dsb
-
-extern "C" int ds_debug_gemm_trace(unsigned long long* dev_buf, int capacity) {
-    dsb::gemm_set_trace(dev_buf, dev_buf ? capacity : 0);
-    return 0;
+int gemm_run(const GemmKernelParams* kp, cudaStream_t stream) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const int slot = (dev < 0 || dev >= 64) ? 0 : dev;
+    if (!g_num_sms[slot]) cudaDeviceGetAttribute(&g_num_sms[slot], cudaDevAttrMultiProcessorCount, slot);
+    switch (kp->BN / 16) {
+        case 1: return gemm_launch<16>(kp, stream, slot);
+        case 2: return gemm_launch<32>(kp, stream, slot);
+        case 3: return gemm_launch<48>(kp, stream, slot);
+        case 4: return gemm_launch<64>(kp, stream, slot);
+        case 5: return gemm_launch<80>(kp, stream, slot);
+        case 6: return gemm_launch<96>(kp, stream, slot);
+        case 7: return gemm_launch<112>(kp, stream, slot);
+        case 8: return gemm_launch<128>(kp, stream, slot);
+        case 9: return gemm_launch<144>(kp, stream, slot);
+        case 10: return gemm_launch<160>(kp, stream, slot);
+        case 11: return gemm_launch<176>(kp, stream, slot);
+        case 12: return gemm_launch<192>(kp, stream, slot);
+        case 13: return gemm_launch<208>(kp, stream, slot);
+        case 14: return gemm_launch<224>(kp, stream, slot);
+        case 15: return gemm_launch<240>(kp, stream, slot);
+        case 16: return gemm_launch<256>(kp, stream, slot);
+        default: return -10;
+    }
 }
+
+}  // namespace dsb
 
 extern "C" int ds_gemm_launch(const ds_gemm_desc* d, cudaStream_t stream) {
     dsb::GemmKernelParams kp;

@@ -9,7 +9,7 @@ extern "C" {
 #endif
 
 // ---------------------------------------------------------------------------------------------
-// Tensor-core GEMM / implicit-GEMM convolution (tcgen05, fp16 operands, fp32 accumulate in TMEM).
+// Tensor-core GEMM / implicit-GEMM convolution (wgmma, fp16 operands, fp32 accumulate in registers).
 //   D[m][n] = sum_k A[m][k] * B[n][k]     (both operands K-major)
 // A is described as a 4-D tensor (c, w, h, n) of fp16 so that one 128-row M tile is a TMA box
 // (64 c, bw, bh, bn) with bw*bh*bn == 128:
@@ -69,8 +69,7 @@ typedef struct ds_gemm_desc {
     const float* rowvec;
     int64_t rowvec_stride;  // elements between samples (0 = broadcast)
     int32_t rows_per_sample;
-    int32_t f8;             // bit 0: fp8 correction passes (see above); requires a_mode == 0, num_z == 1, npass == 3, tap_cb == 0
-                            // bit 1: run this launch on the CTA-pair kernel (gemm_tc_pair_kernel; conv mode, BN % 32 == 0)
+    int32_t f8;             // 1: fp8 correction passes (see above); requires a_mode == 0, num_z == 1, npass == 3, tap_cb == 0
     const float* residual;
     int64_t ldr;
     float scale;
@@ -183,7 +182,7 @@ typedef struct ds_attn_desc {
     int32_t q_pitch, q_c0, k_pitch, k_c0, vt_pitch, o_pitch;
     int32_t nplanes;        // must be 2
     float scale;            // > 0
-    int32_t causal;         // 1: query l attends to keys <= l only (CLIP text encoder; L == Lk).  attn3 kernel only
+    int32_t causal;         // 1: query l attends to keys <= l only (CLIP text encoder; L == Lk)
     int32_t pad0;
 } ds_attn_desc;
 

@@ -1,9 +1,11 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 // Everything here is hand-written PTX; there is no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
+#include "wgmma.cuh"
 
 namespace dsb {
 
@@ -17,10 +19,8 @@ __device__ __forceinline__ uint32_t lane_id() {
     return l;
 }
 
-// One elected lane of a fully converged warp (elect.sync over all 32 lanes).  The tcgen05 issue loops run with the whole warp converged
-// and only the tcgen05.mma / tcgen05.commit instructions elected: when the loop itself sits inside `if (lane == 0)`, ptxas cannot assume
-// convergence and wraps EVERY warp-level tcgen05 instruction in an ELECT / BRA.U.ANY serialisation loop (~75 cycles of single-thread
-// latency per MMA, measured with the attention timeline in profiles/r02): the issue thread, not the tensor pipe, set the pace.
+// One elected lane of a fully converged warp (elect.sync over all 32 lanes): the TMA producer loop runs with the whole warp converged
+// and only the copies elected.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred = 0;
     asm volatile(
@@ -91,176 +91,50 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
         : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, fp32 accumulators in registers)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// Whole warp executes (.sync.aligned). Writes the TMEM base address to *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16/bf16 inputs, fp32 accumulate). One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Same with the A operand in tensor memory (lane = row, two fp16 K elements per 32-bit column: K = 16 is 8 columns).
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Same with e4m3 operands (kind::f8f6f4, K = 32 per instruction, twice the kind::f16 rate); the instruction descriptor of
-// umma_idesc_f16 applies unchanged (format code 0 is F16 for kind::f16 and E4M3 for kind::f8f6f4).
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// Keeps the compiler from moving accumulator accesses across the asynchronous MMAs that own those registers.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major, 128-byte-swizzled operand tile: rows of 128 B (64 x 16-bit), 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// K-major, 128-byte-swizzled operand tile: rows of 128 B (64 x 16-bit or 128 x 8-bit), 8-row groups 1024 B apart.  The tile base
+// must be 1024-byte aligned; a K step of 32 bytes inside the swizzle row adds 2 to the descriptor (16-byte units).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);      // start address, 16-byte units
-    d |= static_cast<uint64_t>(0) << 16;                         // leading byte offset (unused: one swizzle atom along K)
+    d |= static_cast<uint64_t>(1) << 16;                         // leading byte offset (unused: one swizzle atom along K)
     d |= static_cast<uint64_t>(1024 >> 4) << 32;                 // stride byte offset between 8-row groups
-    d |= static_cast<uint64_t>(1) << 46;                         // descriptor version (sm_100)
-    d |= static_cast<uint64_t>(2) << 61;                         // SWIZZLE_128B
+    d |= static_cast<uint64_t>(1) << 62;                         // SWIZZLE_128B
     return d;
 }
-// Instruction descriptor: fp16 x fp16 -> fp32, both operands K-major, M = 128, N runtime (multiple of 16).
-__device__ __forceinline__ uint32_t umma_idesc_f16(uint32_t n) {
-    return (1u << 4) | ((n >> 3) << 17) | ((128u >> 4) << 24);
+
+// D[64 x N] (+)= A * B^T for any N that is a multiple of 16 up to 256: one instruction per set bit of N / 16.  The accumulator
+// of the part starting at column n0 sits at d[n0 / 2 ..], so the register layout is that of a single m64nN instruction; the B part
+// starts n0 rows (n0 * 128 bytes: whole 1024-byte swizzle atoms) further into the tile.
+template <int N, bool F8>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+    static_assert(N % 16 == 0 && N >= 16 && N <= 256, "N");
+    constexpr int n256 = N & 256, n128 = N & 128, n64 = N & 64, n32 = N & 32, n16 = N & 16;
+    auto part = [&](auto nc, int n0) {
+        constexpr int NC = decltype(nc)::value;
+        if (F8) Wgmma<NC>::e4m3(d + n0 / 2, da, db + (uint64_t)(n0 * 128 / 16), scale_d);
+        else Wgmma<NC>::f16(d + n0 / 2, da, db + (uint64_t)(n0 * 128 / 16), scale_d);
+    };
+    if constexpr (n256 != 0) part(std::integral_constant<int, 256>{}, 0);
+    if constexpr (n128 != 0) part(std::integral_constant<int, 128>{}, n256);
+    if constexpr (n64 != 0) part(std::integral_constant<int, 64>{}, n256 + n128);
+    if constexpr (n32 != 0) part(std::integral_constant<int, 32>{}, n256 + n128 + n64);
+    if constexpr (n16 != 0) part(std::integral_constant<int, 16>{}, n256 + n128 + n64 + n32);
 }
 
-// ---------------------------------------------------------------- CTA pair (cta_group::2): two SMs of one TPC execute one 256-row MMA
-// A cluster of two CTAs; rank 0 ("leader") issues the MMAs, both CTAs load operands.  Shared-memory addresses of the two CTAs differ
-// in bit 24 of their shared::cluster form, so `addr & kPeerMask` names the leader's copy of an object from either CTA.
-static constexpr uint32_t kPeerMask = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t cluster_count_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the LEADER CTA's copy of `bar` (callable from both CTAs of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerMask) : "memory");
-}
-// TMA loads of a CTA pair: the bytes land in the executing CTA's shared memory, the transaction count on the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_3d_pair(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerMask), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-// One warp of EACH CTA of the pair executes these (same dst offset in both).
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// 256 x N x 16 (fp16) / 256 x N x 32 (e4m3) MMA over the pair: A rows 0..127 and B rows 0..N/2-1 from the leader's shared memory,
-// the other halves from the same offsets in the peer's; accumulator rows 0..127 in the leader's TMEM, 128..255 in the peer's.
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f8_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// completion of the pair's MMAs arrives on the mbarrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-__device__ __forceinline__ uint32_t umma_idesc_pair(uint32_t n) {          // M = 256 over the pair
-    return (1u << 4) | ((n >> 3) << 17) | ((256u >> 4) << 24);
-}
-
-#define DSB_TMEM_LD_32(taddr, v)                                                                        \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                              \
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "              \
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];" \
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),   \
-                   "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]),            \
-                   "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),         \
-                   "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),         \
-                   "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),         \
-                   "=r"(v[31])                                                                           \
-                 : "r"(taddr) : "memory")
-
-#define DSB_TMEM_LD_16(taddr, v)                                                                        \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                              \
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"        \
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),   \
-                   "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]),            \
-                   "=r"(v[13]), "=r"(v[14]), "=r"(v[15])                                                 \
-                 : "r"(taddr) : "memory")
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// TMEM store: 32 lanes x 32 columns of 32-bit values from this warp's registers (its own lane quadrant), the mirror of DSB_TMEM_LD_32.
-#define DSB_TMEM_ST_32(taddr, v)                                                                        \
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "                                        \
-                 "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "             \
-                 "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"     \
-                 :: "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]),  \
-                    "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]),      \
-                    "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]),   \
-                    "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),   \
-                    "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31]) : "memory")
-
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// named barrier over the 128 threads of one warpgroup (ids 1..; 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 }  // namespace dsb

@@ -319,7 +319,7 @@ extern "C" int ds_update_launch(const ds_update_desc* dp, cudaStream_t stream) {
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!sms[dev]) cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    const long long cap = (long long)(sms[dev] > 0 ? sms[dev] : 148) * 16;
+    const long long cap = (long long)(sms[dev] > 0 ? sms[dev] : 132) * 16;
     const int grid = (int)(blocks < cap ? blocks : cap);
     int rc;
     switch (d.nhist) {

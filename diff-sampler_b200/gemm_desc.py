@@ -1,5 +1,5 @@
 """Builders for ds_gemm_desc (csrc/ops.h): how each contraction of the denoiser maps onto the one
-tcgen05 kernel.  Pure integer/shape logic — importable and testable without a GPU.
+wgmma kernel.  Pure integer/shape logic — importable and testable without a GPU.
 
 Pointer arguments are either absolute device addresses (tests) or plan references (plan.py)."""
 from . import _cstructs as S
@@ -7,22 +7,21 @@ from . import _cstructs as S
 H16 = 2  # bytes per fp16
 
 
-NUM_SMS = 148
+NUM_SMS = 132                            # H100 SXM
 
 
 def _tile_cost(bn):
-    """Duration of one 64-wide K step of a 128 x bn tile, in SM cycles.  Measured (profiles/r02/gemm_tiles_microbench_r02d.txt: 3x3
-    convolutions at 192..1280 channels, every N tile from 64 to 256, fp16x3 and f8): ~690 + bn cycles -- a fixed cost per K step (the
-    16 KB activation tile: 128 rows of 128 B through TMA and the shared-memory port) plus one cycle per weight row; the tensor pipe
-    itself needs 2 x bn, so narrow tiles are far from proportionally cheaper (round 1 modelled max(bn / 2, 32 + bn / 4))."""
+    """Relative cost of one 64-wide K step of a 128 x bn tile: a fixed part per K step (the 16 KB activation tile through TMA and the
+    shared-memory port) plus a part per weight row, so narrow tiles are far from proportionally cheaper.  A tile-selection model,
+    not a measurement."""
     return 690.0 + bn
 
 
 def pick_bn(n):
-    """N tile (UMMA N: any multiple of 16 up to 256): narrow outputs get the smallest covering tile; otherwise the tiling with the least
-    total cost tiles x _tile_cost(bn), ties to less padding: 192 -> 192, 320 -> 160x2, 384 -> 192x2, 576 -> 192x3, 640 -> 224x3 (5 % of
-    zero rows beat a fourth 160-wide tile: measured 411 us with 256x3 against 482 us with 160x4 at 32x32x16 samples), 1280 -> 256x5."""
-    for bn in (32, 64):                  # 32, not 16, for the 3- / 4-channel head convolutions: the CTA-pair kernel (row reuse) needs BN % 32 == 0
+    """N tile (any multiple of 16 up to 256): narrow outputs get the smallest covering tile; otherwise the tiling with the least
+    total cost tiles x _tile_cost(bn), ties to less padding: 192 -> 192, 320 -> 160x2, 384 -> 192x2, 576 -> 192x3, 640 -> 224x3,
+    1280 -> 256x5."""
+    for bn in (32, 64):
         if n <= bn:
             return bn, 1
     best = None
@@ -35,8 +34,8 @@ def pick_bn(n):
 
 
 def fill_bn(n, m_tiles, num_z=1):
-    """N tile for a problem with few tiles (small batch / low resolution): the persistent grid runs ceil(tiles / 148) waves, so
-    160 tiles cost two full waves.  Choose the multiple of 16 that minimises waves x per-tile cost.  Large problems keep pick_bn's tiling.
+    """N tile for a problem with few tiles (small batch / low resolution): the persistent grid runs ceil(tiles / NUM_SMS) waves, so
+    140 tiles cost two full waves.  Choose the multiple of 16 that minimises waves x per-tile cost.  Large problems keep pick_bn's tiling.
     The packed weight keeps pick_bn's padded row count; rows past it are zero-filled by TMA."""
     bn, tiles = pick_bn(n)
     if m_tiles * tiles * num_z >= 4 * NUM_SMS or bn <= 64:
@@ -58,7 +57,7 @@ def split_planes_rows(n_valid, bn):
 
 def conv_box(H, W):
     """TMA box (64, bw, bh, bn) covering 128 consecutive NHWC pixels: whole rows for W <= 128, a 128-pixel row segment for wider
-    images (W a multiple of 128; only the CTA-pair kernel maps tiles to such segments -- conv_gemm requests it)."""
+    images (W a multiple of 128)."""
     if W > 128:
         assert W % 128 == 0, f'unsupported width {W}'
         return 128, 1, 1
@@ -72,7 +71,7 @@ def conv_box(H, W):
 
 def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w_planes=2, a2_ptr=0, C2=0,
               out_f32=0, out_h16=0, o_planes=2, ldo=None, bias=0, rowvec=0, rowvec_stride=0, residual=0, ldr=None, scale=1.0,
-              edm=None, bn=None, s2d=False, f8=False, acc_scale=1.0, pair=False):
+              edm=None, bn=None, s2d=False, f8=False, acc_scale=1.0):
     """3x3 (taps=9) or 1x1 (taps=1) convolution over NHWC fp16 planes [a_planes][Bn][H][W][C] with the
     packed weight matrix [w_planes][Cout_pad][taps*C + C2] (K ordered tap-major, then the aux/skip block).
     Output rows are NHWC pixels: out[pixel][cout] (+ fused epilogue).
@@ -87,11 +86,6 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     d = S.GemmDesc()
     bw, bh, bnn = conv_box(H, W)
     BN, n_tiles = (bn, -(-Cout // bn)) if bn else fill_bn(Cout, -(-(Bn * H * W) // 128))
-    if W > 128:                          # wide rows: pair kernel, whose N tile must split into two 16-row halves
-        pair = True
-        if BN % 32:
-            BN = -(-BN // 32) * 32
-            n_tiles = -(-Cout // BN)
     pbn, ptiles = pick_bn(Cout)
     cout_pad = pbn * ptiles              # rows of the packed weight (pack_conv_weight); tiles past it read TMA zero fill
     ktot = taps * C + C2
@@ -141,7 +135,7 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     d.residual = residual
     d.ldr = ldr if ldr is not None else Cout
     d.scale = scale
-    d.f8 = (1 if f8 else 0) | (2 if pair else 0)        # bit 1: CTA-pair kernel for this launch (opt-in, csrc/ops.h)
+    d.f8 = 1 if f8 else 0
     d.acc_scale = acc_scale
     if edm is not None:
         d.edm_out = 1

@@ -40,8 +40,8 @@ class B200LDMNet:
         self.precision = precision
         self.npass = PRECISIONS[precision]
         self.f8 = precision == 'fp16f8'
-        # with fp16f8, proj_in / attn2.to_q / GEGLU ff / proj_out also run in the f8 GEMM mode (default since round 2: parity green on
-        # hardware, profiles/r02b; DSB_LDM_F8_LINEAR=0 or f8_linear=False keeps them fp16x3)
+        # with fp16f8, proj_in / attn2.to_q / GEGLU ff / proj_out also run in the f8 GEMM mode (held by the f8 parity tests;
+        # DSB_LDM_F8_LINEAR=0 or f8_linear=False keeps them fp16x3)
         if f8_linear is None:
             import os
             f8_linear = os.environ.get('DSB_LDM_F8_LINEAR', '1') != '0'

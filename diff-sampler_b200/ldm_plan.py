@@ -3,7 +3,7 @@
 Reference being lowered: models/ldm/modules/diffusionmodules/openaimodel.py:710-741 (UNetModel.forward), ResBlock :255-275,
 Downsample :134-160, Upsample :91-119; models/ldm/modules/attention.py SpatialTransformer :250-261, BasicTransformerBlock :211-215,
 CrossAttention :170-193, GEGLU :42-44; util.py:151-171 (timestep_embedding).  Same op set and executor as the EDM nets (plan.py):
-every contraction is the tcgen05 GEMM kernel; LayerNorm / GEGLU / softmax / GroupNorm are the HBM-bound companions.
+every contraction is the wgmma GEMM kernel; LayerNorm / GEGLU / softmax / GroupNorm are the HBM-bound companions.
 
 Layout notes specific to this net:
   * head dims 40 / 80 / 160 are zero-padded to 64 / 128 / 192 inside the packed q/k/v/out weights (K blocks are 64 wide);

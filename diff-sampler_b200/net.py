@@ -2,7 +2,7 @@
 
 Drop-in for models.networks_edm.EDMPrecond (networks_edm.py:459-500): same call signature and the attributes the
 samplers and sample.py read (img_resolution, img_channels, label_dim, sigma_min, sigma_max, sigma_data, round_sigma).
-All arithmetic runs in hand-written sm_100a kernels through the C ABI; there is no PyTorch/CPU fallback.
+All arithmetic runs in hand-written sm_90a kernels through the C ABI; there is no PyTorch/CPU fallback.
 """
 import ctypes as C
 from collections import OrderedDict

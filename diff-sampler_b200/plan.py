@@ -302,7 +302,7 @@ def compile_plan(spec, wb, winfo, B, nsig, nlab, npass=3, fuse_stats=True, flash
             emb_buf, emb_rows = 'e3', nE
     if emb_rows >= 32 and ec % 64 == 0:
         # per-sample conditioning (class labels / per-sample sigma): [rows x emb] x [emb x aff_total] is a real GEMM (ImageNet-64 at
-        # batch 256: 20 GFLOP) -> fp16 planes of the embedding (gn_apply in pass-through mode) + the tcgen05 kernel
+        # batch 256: 20 GFLOP) -> fp16 planes of the embedding (gn_apply in pass-through mode) + the wgmma kernel
         A.need('emb_planes', npl * emb_rows * ec * H2)
         emit(lambda R: S.GnApplyDesc(src0=R(emb_buf), src1=0, C0=ec, C1=0, H=emb_rows, W=1, B=1, groups=1, sums=0, gamma=0, beta=0, eps=0.0,
                                      silu=0, ada=0, ada_stride=0, resample=0, nplanes=npl, out_act=0, out_raw=R('emb_planes'), out_raw_f32=0))

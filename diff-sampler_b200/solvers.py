@@ -2,7 +2,7 @@
 
 Same sampler names, argument lists, defaults, return conventions and error behaviour as the reference
 (solvers.py:18-821), so `sample.py` / `fid.py` / `gits_utils.py` can import this module unchanged.  Underneath,
-each step is: one native denoiser evaluation (B200Net, tcgen05 kernels) + ONE fused update kernel that reads the
+each step is: one native denoiser evaluation (B200Net, wgmma kernels) + ONE fused update kernel that reads the
 state, the denoiser output and up to four history buffers and writes the next state and the new history entry.
 No CPU fallback: tensors must be on a CUDA device.
 """

@@ -6,9 +6,9 @@ Reference being lowered (paths under models/ldm/): models/diffusion/ddpm.py:714 
 :82-141 `ResnetBlock` (temb=None), :150-203 `AttnBlock` (one head over all channels), :42-57 `Upsample` (nearest x2 + conv3x3).
 
 Same op set and executor as the denoisers (plan.py / ldm_plan.py): GroupNorm(32, eps 1e-6) statistics + apply(+swish) kernels, the
-tcgen05 GEMM kernel for every convolution (1x1 skip `nin_shortcut` appended along K) and for the QK^T / PV products of the single
+wgmma GEMM kernel for every convolution (1x1 skip `nin_shortcut` appended along K) and for the QK^T / PV products of the single
 wide-head attention, the row softmax.  New for this net: image rows wider than one 128-pixel M tile (256- and 512-wide levels) --
-`gemm_desc.conv_gemm` then requests the CTA-pair GEMM kernel, whose tile -> (w, h, n) mapping handles row segments.
+`gemm_desc.conv_gemm` then tiles them as 128-pixel row segments.
 io slots: X = latents [B, z_ch, R, R] (NCHW fp32), LABELS = coef [1][4] with 1/scale_factor in slot 2, D = images [B, out_ch, sR, sR].
 """
 from collections import OrderedDict

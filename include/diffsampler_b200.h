@@ -1,5 +1,5 @@
 /*
- * diffsampler_b200 — C ABI of the B200-native diffusion ODE sampling hot path.
+ * diffsampler_b200 — C ABI of the CUDA-native (H100, sm_90a) diffusion ODE sampling hot path.
  *
  * The reference (zju-pi/diff-sampler) is pure Python/PyTorch: its hot path has no FFI today.  The
  * boundary it exposes is the Python call surface
@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-/* Library version string, e.g. "diffsampler_b200 0.1 (sm_100a)". */
+/* Library version string, e.g. "diffsampler_b200 0.1 (sm_90a)". */
 const char* ds_version(void);
 /* Text of the last error raised on the calling thread ("" if none). */
 const char* ds_last_error(void);
@@ -113,15 +113,6 @@ int ds_amed_predict(const float* weights, const int* dims6, const float* bottlen
 /* ---- image epilogue: replaces (images * 127.5 + 128).clip(0, 255).to(uint8).permute(0, 2, 3, 1) -------------
  * sample.py:311.  images [B, C, H*W] fp32 NCHW -> out [B, H*W, C] uint8 NHWC (what is written to PNG / gathered for FID). */
 int ds_images_to_uint8(const float* images, unsigned char* out, int B, int C, int HW, void* stream);
-
-/* Debug timeline of the fused attention kernel (profiles/attn_timeline.py): attention ops BUILT after this call make CTA 0 record
- * (tag << 40 | clock) events of its TMA / MMA / softmax roles for its first two tiles into dev_buf[1..capacity) (dev_buf[0] = count,
- * zeroed by the caller).  NULL switches it off.  Not part of the sampling path. */
-int ds_debug_attn_trace(unsigned long long* dev_buf, int capacity);
-/* Debug timeline of the conv / GEMM kernels (profiles/gemm_timeline.py): GEMM launches BUILT after this call make CTA 0 store clock64 per
- * shared-memory ring stage: the TMA producer after its empty-slot wait in dev_buf[i], the MMA warp after its full-slot wait in
- * dev_buf[capacity / 2 + i], i < capacity / 2.  NULL switches it off.  Not part of the sampling path. */
-int ds_debug_gemm_trace(unsigned long long* dev_buf, int capacity);
 
 /* ---- kernel-level entry points (used by the parity tests and micro-benchmarks) ------------------
  * `desc` points to the matching struct of csrc/ops.h with absolute device pointers. */

@@ -140,7 +140,7 @@ def _gemm(mem, d):
         Bn = m_valid // (H * W)
         assert Bn * H * W == m_valid
         if W > 128:
-            assert d.f8 & 2 and W % 128 == 0, 'rows wider than an M tile need the pair kernel'
+            assert W % 128 == 0, 'rows wider than an M tile must be whole 128-pixel segments'
         C = int(d.a_dims[0])
         assert tuple(int(v) for v in d.a_strides) == (C * 2, W * C * 2, H * W * C * 2), 'conv A operand must be dense NHWC'
         taps, cpb = int(d.taps), int(d.cpb)

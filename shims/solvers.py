@@ -1,4 +1,4 @@
-"""Import shim: lets the reference's `import solvers` resolve to the B200-native implementation (see INTEGRATION.md)."""
+"""Import shim: lets the reference's `import solvers` resolve to the CUDA-native implementation (see INTEGRATION.md)."""
 from diff_sampler_b200.solvers import *          # noqa: F401,F403
 from diff_sampler_b200 import solvers as _impl
 

@@ -1,5 +1,5 @@
 """Numerics study (CPU, not a test): final-image error of the f8 GEMM mode on the configuration that misses the 1e-3 gate on the GPU
-(FFHQ-64, iPNDM NFE=6: 1.08e-3 between fp16f8 and fp16x3 at batch 256, profiles/r01d), emulated inside the CPU oracle, with the f8 mode in
+(FFHQ-64, iPNDM NFE=6 with every block in f8), emulated inside the CPU oracle, with the f8 mode in
 all block convolutions and only in those with at least 256 input and output channels (`B200Net(f8_min_channels=256)`).
 
     python tests/study_fp8_sampler.py

@@ -37,7 +37,7 @@ def test_binding_lists_every_declared_symbol(built):
 
 def test_struct_mirrors_and_version(built):
     from diff_sampler_b200 import _lib
-    assert 'sm_100a' in _lib.version()          # load() verifies every sizeof
+    assert 'sm_90a' in _lib.version()          # load() verifies every sizeof
 
 
 def test_no_cpu_fallback(built):

@@ -491,9 +491,8 @@ def test_fused_stats_rejects_partial_slabs(lib):
 # --------------------------------------------------------------------------------------------- fused attention
 @pytest.mark.parametrize('B,nh,L,Lk,d', [(2, 3, 256, 256, 64), (1, 2, 192, 77, 40), (3, 1, 64, 64, 64), (1, 8, 1024, 1024, 40),
                                          (2, 2, 320, 200, 64),
-                                         # round 2 (persistent kernel, two softmax groups over alternate 64-key blocks): more tiles than SMs
-                                         # (192 > 148: CTAs walk several tiles), an odd block count (3), a single block (group 1 idle),
-                                         # many short tiles per CTA (L = 64: 300 tiles)
+                                         # more tiles than SMs (192 > 132), an odd key-block count (3), a single key block,
+                                         # many short tiles (L = 64: 300 tiles)
                                          (4, 6, 1024, 1024, 64), (2, 2, 320, 192, 64), (1, 3, 128, 64, 64), (50, 6, 64, 64, 64), (3, 5, 200, 130, 40)])
 def test_fused_attention(lib, B, nh, L, Lk, d):
     _fused_attention(lib, B, nh, L, Lk, d, causal=False)
@@ -853,79 +852,6 @@ def test_groupnorm_apply_f8_layout(lib, C0, C1, H, W, resample):
         assert e_hi < 6e-4 * m              # fp16: 2^-11 relative
         assert e_sum < 4e-5 * m             # + e4m3 of the residual: 2^-4 of 2^-11
         assert e_h8 < 0.07                  # e4m3: 2^-4 relative
-
-
-# --------------------------------------------------------------------------------------------- CTA-pair GEMM variant
-# (green on hardware since profiles/r01f and r02b; default for the large convolutions since round 2: +2.8 % images/s in the sustained bench)
-
-
-def _time_launch(lib, d, n=5):
-    lib.op_launch(d)
-    sync()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        lib.op_launch(d)
-    e1.record()
-    sync()
-    return e0.elapsed_time(e1) / n
-
-
-@pytest.mark.parametrize('f8', [False, True])
-@pytest.mark.parametrize('Bn,H,W,Cin,Cout,C2', [(80, 32, 32, 256, 256, 0), (75, 32, 32, 64, 128, 64), (300, 16, 16, 128, 192, 0),
-                                                (1185, 8, 8, 128, 128, 0), (3, 16, 16, 128, 256, 0), (20, 64, 64, 192, 192, 0)])
-def test_conv_pair_kernel(lib, f8, Bn, H, W, Cin, Cout, C2):
-    """gemm_tc_pair_kernel (tcgen05.mma.cta_group::2 over a cluster of two CTAs; requested per launch with conv_gemm(pair=True)) against
-    the single-CTA kernel on the same operands and against the references: many tiles, an odd tile count whose last tile is half full
-    (1185 x 8 x 8 -> 593 tiles: phantom tile in the last pair), and a problem smaller than one wave.  The 32 x 32, 16 x 16 and 64 x 64 cases
-    run the row-reuse K loop (halo box of 6 / 10 / 4 rows, with and without the appended 1x1 skip blocks), the 8 x 8 case the plain one."""
-    from diff_sampler_b200 import gemm_desc as G
-    torch.manual_seed(21)
-    x = torch.randn(Bn, Cin, H, W, device=dev())
-    w = torch.randn(Cout, Cin, 3, 3, device=dev()) / (3 * Cin ** 0.5)
-    x2 = torch.randn(Bn, C2, H, W, device=dev()) if C2 else None
-    w2 = torch.randn(Cout, C2, 1, 1, device=dev()) / C2 ** 0.5 if C2 else None
-    bn = 256 if Cout % 256 == 0 else (192 if Cout % 192 == 0 else 128)
-    small = Bn * H * W <= 4096                   # the float64 CPU reference only for the small problem; the large ones are held to the
-    ref = None                                   # single-CTA kernel (itself held to the references by the tests above)
-    if f8:
-        if small:
-            ref, blob, shift, abuf, a2buf = _f8_reference(x, w, x2, w2)
-        else:
-            blob, shift = G.pack_conv_weight_f8(w.cpu(), None if w2 is None else w2.cpu())
-            abuf = G.act_planes_f8(x.permute(0, 2, 3, 1).contiguous())
-            a2buf = G.act_planes_f8(x2.permute(0, 2, 3, 1).contiguous()) if C2 else None
-        wp, xa = blob.to(dev()), abuf.to(dev())
-        x2a = a2buf.to(dev()) if C2 else None
-        tol = 5e-6
-    else:
-        xa = planes(x.permute(0, 2, 3, 1).contiguous())
-        x2a = planes(x2.permute(0, 2, 3, 1).contiguous()) if C2 else None
-        wp = G.pack_conv_weight(w.cpu(), None if w2 is None else w2.cpu()).to(dev())
-        if small:
-            ref = F.conv2d(x.double().cpu(), w.double().cpu(), padding=1)
-            if C2:
-                ref = ref + F.conv2d(x2.double().cpu(), w2.double().cpu())
-        tol = 2e-5
-    ms, outs = {}, {}
-    for pair in (False, True):
-        out = torch.full((Bn * H * W, Cout), float('nan'), device=dev())
-        kw = dict(f8=True, acc_scale=2.0 ** -shift) if f8 else {}
-        d, info = G.conv_gemm(xa.data_ptr(), Bn, H, W, Cin, wp.data_ptr(), Cout, taps=9, npass=3, a2_ptr=x2a.data_ptr() if C2 else 0, C2=C2,
-                              out_f32=out.data_ptr(), bn=bn, pair=pair, **kw)
-        ms[pair] = _time_launch(lib, d)
-        outs[pair] = out
-    scale = outs[False].abs().max().item()
-    dif = (outs[True] - outs[False]).abs().max().item()
-    msg = f'pair conv f8={f8} {Bn}x{H}x{W} {Cin}(+{C2})->{Cout} BN={bn}: single {ms[False] * 1e3:.1f} us, pair {ms[True] * 1e3:.1f} us; pair vs single {dif:.3e}'
-    if ref is not None:
-        ref = ref.permute(0, 2, 3, 1).reshape(Bn * H * W, Cout)
-        err = (outs[True].double().cpu() - ref).abs().max().item()
-        msg += f', pair vs reference {err:.3e}'
-        assert err <= tol * scale
-    print(msg + f' (scale {scale:.2f})')
-    assert not torch.isnan(outs[True]).any()
-    assert dif <= tol * scale
 
 
 # --------------------------------------------------------------------------------------------- LayerNorm / GEGLU writing the f8 operand image

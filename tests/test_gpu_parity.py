@@ -4,7 +4,7 @@
 
 Tolerance (BASELINE.json north_star): max-abs <= 1e-3 per pixel on identical latents/weights.  The weight set is the
 'de-zeroed' random init (|F_x| = O(1)); the reference-init nets (init_zero layers ~1e-5) are a vacuous gate and are
-checked too.  precision='fp16x3' (split-precision tcgen05, 3 MMAs per product) is the mode that must hold 1e-3;
+checked too.  precision='fp16x3' (split-precision wgmma, 3 MMAs per product) is the mode that must hold 1e-3;
 precision='fp16' (single pass) is reported with its own, looser bound.
 """
 import os
@@ -387,7 +387,7 @@ def test_unfused_attention_plan_matches(name):
 
 
 def test_batched_embedding_gemm_path():
-    """>= 32 embedding rows (per-sample labels and sigmas) lower the affine layer to the tcgen05 GEMM instead of the warp-per-feature
+    """>= 32 embedding rows (per-sample labels and sigmas) lower the affine layer to the wgmma GEMM instead of the warp-per-feature
     linear kernel; same tolerance against the oracle."""
     from oracle import edm_oracle as O
     from diff_sampler_b200.net import B200Net

@@ -1,7 +1,7 @@
 """Plans as data, checked without a GPU: the CPU plan interpreter (oracle/plan_interp.py) executes what the plan compilers emit --
 arena offsets, operand planes and formats, packed weights and their scales, tap tables, epilogue options -- and the result must agree
 with the network oracles (which are pinned to the real reference).  The EDM cases double as the interpreter's own validation: those
-plans are the ones the B200 runs green in tests/test_gpu_parity.py."""
+plans are the ones the GPU runs green in tests/test_gpu_parity.py."""
 import pytest
 import torch
 
