@@ -12,6 +12,7 @@ EXPORTS = [
     'ds_version', 'ds_last_error', 'ds_weights_create', 'ds_weights_destroy', 'ds_unet_create', 'ds_unet_destroy',
     'ds_unet_forward', 'ds_unet_debug_read', 'ds_unet_last_launch_count', 'ds_solver_update', 'ds_dyn_threshold',
     'ds_op_launch', 'ds_sizeof', 'ds_unet_set_profiling', 'ds_unet_get_profile', 'ds_unet_op_type', 'ds_gits_cost', 'ds_unet_forward_io', 'ds_images_to_uint8', 'ds_solver_update_u8', 'ds_unet_enable_graph', 'ds_amed_predict',
+    'ds_gemm_config',
 ]
 
 _lib = None
@@ -58,6 +59,7 @@ def load():
     lib.ds_op_launch.argtypes = [C.c_int, vp, sz, vp]
     lib.ds_sizeof.argtypes = [C.c_int]
     lib.ds_sizeof.restype = sz
+    lib.ds_gemm_config.argtypes = [vp, C.POINTER(C.c_int)]
     for which, cls in S.SIZEOF_CHECKS.items():
         got, want = C.sizeof(cls), lib.ds_sizeof(which)
         if got != want:
@@ -80,3 +82,10 @@ def op_launch(desc, stream=0):
     """Launch one kernel-level op from a descriptor struct holding absolute device pointers."""
     lib = load()
     check(lib.ds_op_launch(S.OP_TYPE_OF[type(desc)], C.byref(desc), C.sizeof(desc), C.c_void_p(stream)), type(desc).__name__)
+
+
+def gemm_config(desc):
+    """How the GEMM kernel runs a GemmDesc on the current device: dict(stages, grid)."""
+    info = (C.c_int * 2)()
+    check(load().ds_gemm_config(C.byref(desc), info), 'ds_gemm_config')
+    return dict(stages=info[0], grid=info[1])

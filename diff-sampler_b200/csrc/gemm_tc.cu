@@ -26,7 +26,7 @@ namespace dsb {
 static constexpr int kMaxStages = 8;
 static constexpr int kATileBytes = 128 * 128;   // 128 rows x 64 fp16 (or 128 e4m3)
 static constexpr int kThreads = 384;           // warpgroup 0: producer (warp 0), 1 and 2: consumers
-static constexpr int kStgPitch = 68;           // floats per row of the epilogue staging buffer (64 columns + 4: conflict-free row reads)
+static constexpr int kStgPitch = 64;           // floats per row of the epilogue staging buffer (16-byte chunks XOR-swizzled: stg_swz)
 static constexpr int kStgBytes = 2 * 64 * kStgPitch * 4;
 static constexpr int kSmemLimit = 227 * 1024;
 
@@ -406,39 +406,63 @@ __device__ __forceinline__ void mma_tile(const GemmKernelParams& p, uint8_t* sme
 // Accumulator fragment (m64nBN): register g of lane L in warp w holds row 16 w + L / 4 + 8 ((g >> 1) & 1), column 8 (g / 4) + 2 (L % 4)
 // + (g & 1).  Per 64-column chunk the warpgroup stages its 64 x 64 block in shared memory; then warp w takes rows 32 (w & 1) + lane
 // (one row per lane: the layout epilogue_chunk expects, 32-row slabs for the GroupNorm partials) and columns 32 (w >> 1) .. + 32.
+//
+// Staging rows are 64 floats (256 bytes) with no padding; the 16-byte chunk c of row r is stored at chunk c ^ f(r & 7),
+// f = {0,2,4,6,1,3,5,7}.  Fragment stores (float2): each half warp writes 4 rows x 2 adjacent chunks {2i, 2i+1}; f(r) >> 1 differs
+// across those rows, so the 8 chunks land in 8 different bank groups.  Row reads (float4): each quarter warp reads one chunk of 8
+// consecutive rows; f is a permutation of 0..7, so again 8 different bank groups.  An address is a per-row key (row base + f) with
+// the in-row offset XORed on: rows are 256-byte aligned and no in-row offset carries into bit 8.  Without the padding the ring
+// gets one more stage at BN = 256 (4) and at BN = 128 (6).
+__device__ __forceinline__ uint32_t stg_swz(uint32_t r) { return (((r & 3) << 1) | ((r >> 2) & 1)) << 4; }
+
+// The lane id, re-read wherever it is used: the staging keys derived from it are then rebuilt per chunk instead of being held in
+// registers across the whole epilogue (at BN = 256 the accumulators leave no room for them).
+__device__ __forceinline__ uint32_t lane_id_here() {
+    uint32_t l;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+    return l;
+}
+__device__ __forceinline__ void sts_f2(uint32_t a, float x, float y) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float4 lds_f4(uint32_t a) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+    return v;
+}
+
 template <int BN>
 __device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, float* stg, const int wg, const TileCoord& tc, const float (&acc)[BN / 2]) {
     const int lane = threadIdx.x & 31;
     const int w = (threadIdx.x >> 5) & 3;
-    const int frag_row = 16 * w + (lane >> 2);
     const int row = 32 * (w & 1) + lane;
     const long long grow = (long long)tc.mt * 128 + wg * 64 + row;
     const bool row_ok = grow < p.m_valid;
+    const int ch = 32 * (w >> 1);
 #pragma unroll
     for (int c0 = 0; c0 < BN; c0 += 64) {
+        uint32_t ln = lane_id_here();
+        // fragment row 16 w + ln / 4 (+ 8), columns 8 i + 2 (ln % 4): (row & 7) == ln / 4
+        const uint32_t wkey = smem_u32(stg) + (16 * w + (ln >> 2)) * 256 + ((8 * (ln & 3)) ^ stg_swz(ln >> 2));
 #pragma unroll
         for (int g = 0; g < 32; g += 2) {
             const int gi = c0 / 2 + g;
-            if (gi < BN / 2) {
-                const int col = 8 * (g >> 2) + 2 * (lane & 3);
-                const int rr = frag_row + 8 * ((g >> 1) & 1);
-                *reinterpret_cast<float2*>(stg + rr * kStgPitch + col) = make_float2(acc[gi], acc[gi + 1]);
-            }
+            if (gi < BN / 2) sts_f2((wkey + 2048 * ((g >> 1) & 1)) ^ (32 * (g >> 2)), acc[gi], acc[gi + 1]);
         }
         warpgroup_sync(1 + wg);
-        const int ch = 32 * (w >> 1);
         const int width = min(32, BN - c0 - ch);
         const int col0 = tc.nt * BN + c0 + ch;
-        const float* src = stg + row * kStgPitch + ch;
+        ln = lane_id_here();
+        const uint32_t rkey = smem_u32(stg) + (32 * (w & 1) + ln) * 256 + 4 * ch + stg_swz(ln);      // (row & 7) == ln % 8
         if (width >= 32) {
             float v[32];
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(v + j) = *reinterpret_cast<const float4*>(src + j);
+            for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(v + j) = lds_f4(rkey ^ (4 * j));
             if (col0 < p.n_valid) epilogue_chunk<32>(p, v, grow, col0, row_ok, tc.zb, tc.zh, nullptr, false);
         } else if (width >= 16) {
             float v[16];
 #pragma unroll
-            for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(v + j) = *reinterpret_cast<const float4*>(src + j);
+            for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(v + j) = lds_f4(rkey ^ (4 * j));
             if (col0 < p.n_valid) epilogue_chunk<16>(p, v, grow, col0, row_ok, tc.zb, tc.zh, nullptr, false);
         }
         warpgroup_sync(1 + wg);
@@ -699,4 +723,17 @@ extern "C" int ds_gemm_launch(const ds_gemm_desc* d, cudaStream_t stream) {
     int rc = dsb::gemm_build(d, &kp);
     if (rc) return rc;
     return dsb::gemm_run(&kp, stream);
+}
+
+extern "C" int ds_gemm_config(const void* desc, int* info) {
+    dsb::GemmKernelParams kp;
+    int rc = dsb::gemm_build(static_cast<const ds_gemm_desc*>(desc), &kp);
+    if (rc) return rc;
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -20;
+    const int tiles = kp.num_z * kp.m_tiles * kp.n_tiles;
+    info[0] = kp.num_stages;
+    info[1] = tiles < sms ? tiles : sms;
+    return 0;
 }

@@ -119,6 +119,9 @@ int ds_images_to_uint8(const float* images, unsigned char* out, int B, int C, in
 int ds_op_launch(int op_type, const void* desc, size_t desc_size, void* stream);
 /* sizeof() of the descriptor structs as compiled (0 = ds_plan_op, else DS_OP_* code); lets bindings verify their mirrors. */
 size_t ds_sizeof(int which);
+/* How the GEMM kernel would run `desc` (a ds_gemm_desc) on the current device: info[0] shared-memory ring stages, info[1] CTAs in
+ * the persistent grid. */
+int ds_gemm_config(const void* desc, int* info);
 
 #ifdef __cplusplus
 }
