@@ -350,8 +350,13 @@ __device__ __forceinline__ void producer_tile(const GemmKernelParams& p, uint8_t
             for (int j = 0; j < p.nkb8_aux; ++j, bk += 128) load(&p.tmA2_8, j * 128, aw0, ah0, an8, &p.tmB8, bk, pass8);
         }
     }
-    const int npass16 = p.f8 ? 1 : p.npass;                 // fp16 passes: hi x hi (, lo x hi, hi x lo)
-    for (int pass = 0; pass < npass16; ++pass) {
+    // fp16 passes: (lo x hi, hi x lo,) then hi x hi.  Every wgmma adds an error proportional to the accumulator's current
+    // magnitude (on H100 the fp32 accumulation error grows linearly with K), so the two small correction products go first, while
+    // the sum is still ~2^-11 of its final size, as the e4m3 corrections do in f8 mode; only the main product then accumulates at
+    // full magnitude.
+    const int npass16 = p.f8 ? 1 : p.npass;
+    for (int pi = 0; pi < npass16; ++pi) {
+        const int pass = npass16 == 3 ? (pi + 1) % 3 : pi;
         const int an = an0 + (pass == 1 ? p.a_plane_n : 0);
         const int an2 = an0 + (pass == 1 ? p.a2_plane_n : 0);
         const int bz = b_z + (pass == 2 ? p.b_plane_batch : 0);

@@ -16,7 +16,7 @@ extern "C" {
 //   a_mode 0 (conv):  rows are NHWC pixels; a 3x3 tap is a shifted box, halo zero-filled by TMA.
 //   a_mode 1 (rows):  plain row-major matrices, optionally batched over z = (zb, zh).
 // B is a 3-D tensor (k, row, batch).  Split precision: npass == 3 accumulates
-//   A_hi*B_hi + A_lo*B_hi + A_hi*B_lo, with the 'lo' planes found at a_plane_n / b_plane_batch.
+//   A_lo*B_hi + A_hi*B_lo + A_hi*B_hi (the small corrections first), with the 'lo' planes found at a_plane_n / b_plane_batch.
 //
 // f8 == 1 ("fp16f8", conv mode only): the two correction products run as e4m3 MMAs (kind::f8f6f4, twice the fp16 rate, 128
 // channels per K block).  Operand layout (all scales are powers of two, so the fp16 roundings are those of the unscaled values):

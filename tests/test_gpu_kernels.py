@@ -753,25 +753,26 @@ def test_image_epilogue_uint8_bit_exact(lib):
 
 # --------------------------------------------------------------------------------------------- f8 GEMM mode (fp16 hi x hi + e4m3 corrections)
 def _f8_reference(x, w, x2=None, w2=None):
-    """What the f8 GEMM computes, in float64 from the decoded operand planes (csrc/ops.h): hi x hi + lo8 x w_hi8 + hi8 x w_lo8."""
+    """What the f8 GEMM computes, in float64 from the decoded operand planes (csrc/ops.h): hi x hi + lo8 x w_hi8 + hi8 x w_lo8.
+    The operands are packed and decoded on the host; the convolutions run on x's device."""
     from diff_sampler_b200 import gemm_desc as G
     Cout, Cin = w.shape[0], w.shape[1]
     taps = w.shape[2] * w.shape[3]
     blob, shift = G.pack_conv_weight_f8(w.cpu(), None if w2 is None else w2.cpu())
     (m16, s16), (mh8, sh8), (ml8, sl8) = G.decode_conv_weight_f8(blob, shift, Cout, Cin, taps, 0 if w2 is None else w2.shape[1])
     k = w.shape[2]
-    as_w = lambda m: m.reshape(Cout, k, k, Cin).permute(0, 3, 1, 2).double()
+    as_w = lambda m: m.reshape(Cout, k, k, Cin).permute(0, 3, 1, 2).to(x.device).double()
     xn = x.permute(0, 2, 3, 1).contiguous().cpu()
     abuf = G.act_planes_f8(xn)
-    hi, lo8, hi8 = [t.permute(0, 3, 1, 2).double() for t in G.decode_act_planes_f8(abuf, xn.shape)]
+    hi, lo8, hi8 = [t.permute(0, 3, 1, 2).to(x.device).double() for t in G.decode_act_planes_f8(abuf, xn.shape)]
     pad = k // 2
     ref = F.conv2d(hi, as_w(m16), padding=pad) + F.conv2d(lo8, as_w(mh8), padding=pad) + F.conv2d(hi8, as_w(ml8), padding=pad)
     a2buf = None
     if w2 is not None:
         x2n = x2.permute(0, 2, 3, 1).contiguous().cpu()
         a2buf = G.act_planes_f8(x2n)
-        h2, l2, h82 = [t.permute(0, 3, 1, 2).double() for t in G.decode_act_planes_f8(a2buf, x2n.shape)]
-        as_s = lambda m: m.reshape(Cout, -1, 1, 1).double()
+        h2, l2, h82 = [t.permute(0, 3, 1, 2).to(x.device).double() for t in G.decode_act_planes_f8(a2buf, x2n.shape)]
+        as_s = lambda m: m.reshape(Cout, -1, 1, 1).to(x.device).double()
         ref = ref + F.conv2d(h2, as_s(s16)) + F.conv2d(l2, as_s(sh8)) + F.conv2d(h82, as_s(sl8))
     return ref, blob, shift, abuf, a2buf
 
@@ -802,7 +803,7 @@ def test_conv_f8_mode(lib, Bn, H, W, Cin, Cout, C2, taps):
     to_rows = lambda t: t.permute(0, 2, 3, 1).reshape(Bn * H * W, Cout)
     got = out.double().cpu()
     scale = exact.abs().max().item()
-    e_model = (got - to_rows(ref)).abs().max().item()
+    e_model = (got - to_rows(ref.cpu())).abs().max().item()
     e_exact = (got - to_rows(exact)).abs().max().item()
     print(f'conv f8 {Bn}x{H}x{W} {Cin}(+{C2})->{Cout} taps{taps} BN={info["BN"]} S={shift}: vs operand model {e_model:.3e}, vs exact {e_exact:.3e} '
           f'(scale {scale:.2f})')

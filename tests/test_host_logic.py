@@ -391,3 +391,19 @@ def test_solver_update_rejects_missing_history_and_miscounted_coefficients():
         U.solver_update(x, x, [1.0, 0.0, 0.5], hist=[None])
     with pytest.raises(ValueError, match='coefficients'):
         U.solver_update(x, x, [1.0, 0.0, 0.5, 0.5], hist=[x])
+
+
+def test_benchmark_plans_cover_the_gemm_tile_configurations():
+    """tests/test_gpu_gemm_tiles.py replays every GEMM configuration of the benchmarked plans against float64.  The EDM plans at the
+    benchmark's batch and precision must keep offering it the cases that matter: N tiles 32 to 256, f8 blocks whose last 128-channel
+    e4m3 block is half empty, both statistics granularities, the EDM output fold and rows mode."""
+    from diff_sampler_b200 import gemm_replay
+    cfgs = set()
+    for name, B, fmin in (('cifar10', 512, 0), ('ffhq', 256, 256), ('imagenet64', 256, 0)):
+        cfgs |= set(gemm_replay.plan_configs(gemm_replay.edm_plan(name, B, fmin)))
+    assert {c.BN for c in cfgs} >= {32, 64, 128, 192, 256}
+    assert any(c.f8 and ((c.C // 64) % 2 or (c.C2 // 64) % 2) for c in cfgs)
+    assert {c.st_unit for c in cfgs} >= {2, 4}
+    assert any(c.edm == 1 for c in cfgs)
+    assert any(c.mode == 'rows' for c in cfgs)
+    assert any(c.f8 and c.BN in (192, 256) for c in cfgs)

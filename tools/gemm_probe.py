@@ -3,11 +3,12 @@
 
     python tools/gemm_probe.py [--root TREE] [--batch 512] [--seconds 0.5] [--out FILE.json]
 
-Every distinct convolution shape of the compiled plan is rebuilt with gemm_desc.conv_gemm on seeded device buffers and launched
+Every distinct GEMM configuration of the compiled plan is rebuilt by gemm_replay.make_desc on seeded device buffers and launched
 alone, CUDA events around >= --seconds of back-to-back launches after warm-up.  Per shape: ms per launch, algorithmic TFLOP/s
 (2 M N K), and the bytes the CTAs request from L2 into shared memory per launch (every ring stage of every tile: one A box and one
 B box), with their rate.  The dominant shape is also run at BN = 128 and BN = 256: if its time followed those bytes rather than its
-FLOPs, L2 bandwidth would be the limit.  --root imports the package from another checkout of this project (to compare builds in one run)."""
+FLOPs, L2 bandwidth would be the limit.  --root imports the package and library from another checkout of this project (to compare
+builds in one run); the configurations are always rebuilt by this checkout's gemm_replay, on top of that checkout's gemm_desc."""
 import argparse
 import json
 import os
@@ -26,61 +27,26 @@ def gpu_info():
         return dict(error=repr(e))
 
 
+def replay_module():
+    """This checkout's gemm_replay, loaded into the imported package (which --root may take from an older checkout without it)."""
+    import importlib.util
+    name = 'diff_sampler_b200.gemm_replay'
+    if name not in sys.modules:
+        spec = importlib.util.spec_from_file_location(name, os.path.join(ROOT, 'diff-sampler_b200', 'gemm_replay.py'))
+        mod = importlib.util.module_from_spec(spec)
+        sys.modules[name] = mod
+        spec.loader.exec_module(mod)
+    return sys.modules[name]
+
+
 def plan_shapes(net, B, dev):
-    """Distinct implicit-GEMM convolutions of one forward: (key -> dict(desc fields, launches per forward))."""
+    """Distinct GEMM configurations of one forward (gemm_replay.GemmCfg -> launches per forward)."""
     import torch
-    from diff_sampler_b200 import _cstructs as S
+    gemm_replay = replay_module()
     x = torch.randn(B, net.img_channels, net.img_resolution, net.img_resolution, device=dev)
     net(x, torch.tensor(2.0, device=dev))
     _, pl = next(iter(net._plans.values()))
-    shapes = {}
-    for i in range(pl.n_ops):
-        op = pl.ops_array[i]
-        if op.type != S.DS_OP_GEMM:
-            continue
-        d = op.u.gemm
-        if d.a_mode != 0:
-            continue
-        key = (int(d.taps), int(d.cpb) * 64, int(d.a2_c), int(d.n_valid), int(d.conv_H), int(d.conv_W), int(d.m_valid), int(d.BN),
-               bool(d.f8 & 1), int(d.npass), bool(d.out_f32), bool(d.out_h16), bool(d.st_quads))
-        ent = shapes.setdefault(key, dict(n=0))
-        ent['n'] += 1
-    return shapes
-
-
-def make_desc(key, dev, bn=None):
-    """conv_gemm descriptor of one plan shape on seeded buffers (kept alive in the returned list)."""
-    import torch
-    from diff_sampler_b200 import gemm_desc as G
-    taps, C, C2, N, H, W, M, BN, f8, npass, o32, o16, stq = key
-    Bn = M // (H * W)
-    g = torch.Generator().manual_seed(0)
-    k = 3 if taps == 9 else 1
-    x = torch.randn(Bn, H, W, C, generator=g)
-    w = torch.randn(N, C, k, k, generator=g) / (k * C ** 0.5)
-    x2 = torch.randn(Bn, H, W, C2, generator=g) if C2 else None
-    w2 = torch.randn(N, C2, 1, 1, generator=g) / max(C2, 1) ** 0.5 if C2 else None
-    bn = bn or BN
-    keep = []
-    # weights packed at pick_bn's row count, as the plan packs them (conv_gemm's B extent); other N tiles read TMA zero fill
-    if f8:
-        blob, shift = G.pack_conv_weight_f8(w, w2)
-        a, a2 = G.act_planes_f8(x), (G.act_planes_f8(x2) if C2 else None)
-        acc = 2.0 ** -shift
-    else:
-        blob, acc = G.pack_conv_weight(w, w2), 1.0
-        a, a2 = G.split_planes(x), (G.split_planes(x2) if C2 else None)
-    keep += [t.to(dev) for t in (blob, a) + ((a2,) if C2 else ())]
-    out = torch.empty(M, N, device=dev)
-    outh = torch.empty(2, M, N, dtype=torch.float16, device=dev) if o16 else None
-    quads = torch.empty(M // 32, N // 2, 2, device=dev) if stq else None
-    keep += [t for t in (out, outh, quads) if t is not None]
-    d, info = G.conv_gemm(keep[1].data_ptr(), Bn, H, W, C, keep[0].data_ptr(), N, taps=taps, npass=3 if f8 else npass,
-                          a2_ptr=keep[2].data_ptr() if C2 else 0, C2=C2, out_f32=out.data_ptr(), out_h16=outh.data_ptr() if o16 else 0,
-                          f8=f8, acc_scale=acc, bn=bn)
-    if stq:
-        d.st_quads = quads.data_ptr()
-    return d, info, keep
+    return gemm_replay.plan_configs(pl)
 
 
 def l2_bytes(d):
@@ -128,6 +94,7 @@ def main():
     from diff_sampler_b200 import _lib as L
     from diff_sampler_b200 import gemm_desc as G
     from diff_sampler_b200.net import B200Net
+    make_desc = replay_module().make_desc
     assert torch.cuda.is_available(), 'the probe times kernels on a CUDA device'
     dev = torch.device('cuda:0')
     gpu = gpu_info()
@@ -143,10 +110,10 @@ def main():
         ms, n = time_launch(L, d, args.seconds)
         r = G.describe(d)
         by, stages = l2_bytes(d)
-        row = dict(label=r['label'], BN=int(d.BN), launches_per_forward=shapes.get(key, {}).get('n', 0), ms=ms, timed_launches=n,
+        row = dict(label=r['label'], BN=int(d.BN), launches_per_forward=shapes[key], ms=ms, timed_launches=n,
                    tflops=r['flops'] / (ms / 1e3) / 1e12, k_stages_per_tile=stages, l2_smem_bytes=by, l2_smem_tbs=by / (ms / 1e3) / 1e12,
                    ring_stages=cfg['stages'] if cfg else None, grid=cfg['grid'] if cfg else None,
-                   fwd_ms=ms * shapes.get(key, {}).get('n', 0))
+                   fwd_ms=ms * shapes[key])
         rows.append(row)
         del keep
         if dom is None or row['fwd_ms'] > dom[1]['fwd_ms']:
