@@ -57,14 +57,27 @@ def plan_configs(pl):
     return out
 
 
-def edm_plan(name, B, f8_min_channels=0, seed=0):
-    """The fp16f8 plan B200Net compiles for an EDM net at batch B (one sigma for the batch, a label per sample), on the host."""
+def edm_plan(name, B, f8_min_channels=0, seed=0, dezero=False, norm_jitter=False, with_weights=False):
+    """The fp16f8 plan B200Net compiles for an EDM net at batch B (one sigma for the batch, a label per sample), on the host.
+    dezero: the weight set bench.py runs (edm_nets.dezero_); norm_jitter: seeded per-channel GroupNorm gains 1 + U(-0.1, 0.1) and
+    biases U(-0.1, 0.1) instead of the init's ones and zeros, so that the channels of a group get different coefficients;
+    with_weights: return (plan, weight blob bytes)."""
+    import torch
     from . import edm_nets, plan as planner
     params, cfg = edm_nets.init_params(name, seed=seed)
+    if dezero:
+        edm_nets.dezero_(params, cfg['kind'], seed=seed)
+    if norm_jitter:
+        g = torch.Generator().manual_seed(seed + 4242)
+        for k in params:
+            if 'norm' in k.rsplit('.', 2)[-2] and params[k].dim() == 1:
+                u = torch.rand(params[k].shape, generator=g) * 0.2 - 0.1
+                params[k] = (1.0 + u) if k.endswith('.weight') else u
     spec = edm_nets.spec_from_params(params, cfg['img_resolution'], cfg['img_channels'], cfg.get('label_dim', 0))
     spec.sigma_data = 0.5
     wb, info = planner.pack_weights(spec, params, f8=True, f8_min_channels=f8_min_channels)
-    return planner.compile_plan(spec, wb, info, B, 1, B if spec.label_dim else 0, npass=3, f8=True)
+    pl = planner.compile_plan(spec, wb, info, B, 1, B if spec.label_dim else 0, npass=3, f8=True)
+    return (pl, wb.bytes()) if with_weights else pl
 
 
 def tiles_of(cfg, batch=None):

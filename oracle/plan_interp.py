@@ -21,10 +21,18 @@ F8_A16, F8_LO8, F8_HI8 = S.DS_F8_SH_A16, S.DS_F8_SH_LO8, S.DS_F8_SH_HI8
 
 
 class Memory:
-    def __init__(self, arena_bytes, weight_blob, io):
-        self.arena = torch.zeros(int(arena_bytes), dtype=torch.uint8)
-        self.weights = torch.frombuffer(bytearray(weight_blob), dtype=torch.uint8)
+    """The three address spaces of a plan.  By default a zeroed host arena and a host copy of the weight blob; `device` places them
+    elsewhere, and `arena` / `weights` (uint8 tensors) wrap existing buffers instead (e.g. a live device arena or a snapshot of it).
+    Every tensor an op creates is made on `device`.  `stored`, when a list, receives (ref, fmt, float64 values, index) for every
+    fp16-plane or f8-image store: the values before they are rounded into the planes."""
+    def __init__(self, arena_bytes, weight_blob, io, device='cpu', arena=None, weights=None):
+        self.device = torch.device(device)
+        self.arena = torch.zeros(int(arena_bytes), dtype=torch.uint8, device=self.device) if arena is None else arena
+        if weights is None:
+            weights = torch.frombuffer(bytearray(weight_blob), dtype=torch.uint8).to(self.device)
+        self.weights = weights
         self.io = io                                           # slot -> contiguous torch tensor (fp32) or None
+        self.stored = None
 
     def raw(self, ref):
         ref = int(ref)
@@ -81,6 +89,8 @@ def _store_planes(mem, ref, values, nplanes, fmt=0, plane_elems=None, index=None
     v = values.reshape(-1).to(torch.float64)
     n = v.numel() if plane_elems is None else int(plane_elems)
     idx = slice(None) if index is None else index.reshape(-1)
+    if mem.stored is not None:
+        mem.stored.append((int(ref), fmt, v, index))
     if fmt == 0:
         hi = v.to(torch.float32).to(torch.float16)
         mem.view(ref, torch.float16, n)[idx] = hi
@@ -119,7 +129,7 @@ def _im2col(x, d, cpb_ch, taps, use_taps=True):
     cols = []
     for t in range(taps):
         dh, dw, cb = (int(d.tap_dh[t]), int(d.tap_dw[t]), int(d.tap_cb[t])) if use_taps else (0, 0, 0)
-        sh = torch.zeros(Bn, H, W, cpb_ch, dtype=x.dtype)
+        sh = torch.zeros(Bn, H, W, cpb_ch, dtype=x.dtype, device=x.device)
         h0, h1 = max(0, -dh), min(H, H - dh)
         w0, w1 = max(0, -dw), min(W, W - dw)
         cc = max(0, min(cpb_ch, C - cb))
@@ -174,7 +184,7 @@ def _gemm(mem, d):
                 bl = mem.view(d.b_ptr, torch.float16, rows_b * ktot, byte_offset=int(d.b_strides[1]) * int(d.b_plane_batch)).reshape(rows_b, ktot).double()
                 acc = acc + amat('lo', cpb * 64) @ bh[:nrows].T + amat('hi', cpb * 64) @ bl[:nrows].T
         if nrows < n_valid:
-            acc = torch.cat([acc, torch.zeros(m_valid, n_valid - nrows, dtype=acc.dtype)], dim=1)
+            acc = torch.cat([acc, torch.zeros(m_valid, n_valid - nrows, dtype=acc.dtype, device=acc.device)], dim=1)
         results.append(acc)
     else:
         assert not f8
@@ -189,7 +199,7 @@ def _gemm(mem, d):
         bbuf = mem.view(d.b_ptr, torch.float16, (b_tot - 1) * b_bstride + b_rows * b_pitch)
 
         def a_block(batch, c_off):
-            x = torch.zeros(m_valid, K, dtype=torch.float64)
+            x = torch.zeros(m_valid, K, dtype=torch.float64, device=mem.device)
             rows = min(m_valid, a_rows)
             cc = max(0, min(K, a_kv - c_off))
             if cc > 0:
@@ -197,7 +207,7 @@ def _gemm(mem, d):
             return x
 
         def b_block(batch, k_off, row_off):
-            x = torch.zeros(n_valid, K, dtype=torch.float64)
+            x = torch.zeros(n_valid, K, dtype=torch.float64, device=mem.device)
             rows = max(0, min(n_valid, b_rows - row_off))
             cc = max(0, min(K, b_kv - k_off))
             if rows > 0 and cc > 0:
@@ -215,7 +225,7 @@ def _gemm(mem, d):
             results.append(acc)
     # ---- epilogue -------------------------------------------------------------------------------------------------------------
     acc_scale = float(d.acc_scale) if d.acc_scale else 1.0
-    rows = torch.arange(m_valid)
+    rows = torch.arange(m_valid, device=mem.device)
     for z, acc in enumerate(results):
         zb, zh = divmod(z, nh)
         r = acc * acc_scale
@@ -295,7 +305,7 @@ def _gn_finalize(mem, d):
         # per-channel view of the partials (each unit's sums attributed to its first channel) so that any grouping can be summed
         def per_channel(ptr, Cx, u):
             q = mem.view(ptr, torch.float32, B * slabs * (Cx // u) * 2).reshape(B, slabs, Cx // u, 2).double().sum(dim=1)
-            out = torch.zeros(B, Cx, 2, dtype=torch.float64)
+            out = torch.zeros(B, Cx, 2, dtype=torch.float64, device=mem.device)
             out[:, ::u, :] = q
             return out
         pc = per_channel(d.quads0, C0, u0)
@@ -394,7 +404,7 @@ def _posemb(mem, d):
     n, ch = int(d.nsig), int(d.num_channels)
     sig = mem.view(d.sigma, torch.float32, n).double()
     half = ch // 2
-    i = torch.arange(half, dtype=torch.float64)
+    i = torch.arange(half, dtype=torch.float64, device=mem.device)
     emb = mem.view(d.emb, torch.float32, n * ch).reshape(n, ch)
     if d.mode == 1:
         a = sig[:, None] * torch.exp(-math.log(10000.0) * i / half)[None, :]
@@ -436,7 +446,7 @@ def _prep_input(mem, d):
     x = mem.view(d.x, torch.float32, xb * C * HW).reshape(xb, C, HW).double()
     cst = int(d.coef_stride)
     coef = mem.view(d.coef, torch.float32, (xb - 1) * cst + 4)
-    out = torch.zeros(B, HW, 64, dtype=torch.float64)
+    out = torch.zeros(B, HW, 64, dtype=torch.float64, device=mem.device)
     for n in range(B):
         nx = n % xb
         out[n, :, :C] = (float(coef[nx * cst + 2]) * x[nx]).T
@@ -478,13 +488,13 @@ def _attn(mem, d):
     q = _planes_f16(mem, d.q, B * L * qp, 2).reshape(B, L, qp)
     k = _planes_f16(mem, d.k, B * Lk * kp, 2).reshape(B, Lk, kp)
     vt = _planes_f16(mem, d.vt, B * nh * 64 * vp, 2).reshape(B, nh * 64, vp)
-    out = torch.zeros(B, L, op, dtype=torch.float64)
+    out = torch.zeros(B, L, op, dtype=torch.float64, device=mem.device)
     for h in range(nh):
         qs = q[:, :, int(d.q_c0) + h * 64:int(d.q_c0) + (h + 1) * 64]
         ks = k[:, :, int(d.k_c0) + h * 64:int(d.k_c0) + (h + 1) * 64]
         sc = float(d.scale) * qs @ ks.transpose(1, 2)
         if int(d.causal):
-            sc = sc + torch.full((L, Lk), float('-inf'), dtype=torch.float64).triu(1)
+            sc = sc + torch.full((L, Lk), float('-inf'), dtype=torch.float64, device=mem.device).triu(1)
         p = torch.softmax(sc, dim=2)
         out[:, :, h * 64:(h + 1) * 64] = p @ vt[:, h * 64:(h + 1) * 64, :Lk].transpose(1, 2)
     idx = None
@@ -498,7 +508,7 @@ def _embed(mem, d):
     ids = mem.view(d.ids, torch.int32, rows).long().clamp(0, V - 1)
     tok = mem.view(d.tok, torch.float32, V * C_).reshape(V, C_)
     pos = mem.view(d.pos, torch.float32, T * C_).reshape(T, C_)
-    mem.view(d.out, torch.float32, rows * C_)[:] = (tok[ids] + pos[torch.arange(rows) % T]).reshape(-1)
+    mem.view(d.out, torch.float32, rows * C_)[:] = (tok[ids] + pos[torch.arange(rows, device=mem.device) % T]).reshape(-1)
 
 
 _DISPATCH = {
@@ -510,18 +520,22 @@ _DISPATCH = {
 }
 
 
+def run_op(mem, op):
+    """Execute one ds_plan_op (pointer fields still plan references) on `mem`."""
+    with torch.no_grad():
+        if op.type == S.DS_OP_MEMSET:
+            mem.view(op.u.memset.ptr, torch.uint8, int(op.u.memset.bytes))[:] = 0
+            return
+        field, fn = _DISPATCH[op.type]
+        fn(mem, getattr(op.u, field))
+
+
 def run_plan(plan, weight_blob, io):
     """Execute `plan` (diff_sampler_b200.plan.Plan) on the host.  io: {DS_IO_* slot: contiguous fp32 CPU tensor}; output tensors
     (e.g. DS_IO_D) are written in place.  Returns the Memory (arena readable through plan.arena_offsets)."""
     mem = Memory(plan.arena_bytes, weight_blob, io)
-    with torch.no_grad():
-        for i in range(plan.n_ops):
-            op = plan.ops_array[i]
-            if op.type == S.DS_OP_MEMSET:
-                mem.view(op.u.memset.ptr, torch.uint8, int(op.u.memset.bytes))[:] = 0
-                continue
-            field, fn = _DISPATCH[op.type]
-            fn(mem, getattr(op.u, field))
+    for i in range(plan.n_ops):
+        run_op(mem, plan.ops_array[i])
     return mem
 
 

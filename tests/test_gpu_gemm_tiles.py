@@ -302,21 +302,35 @@ _REPLAYED = set()
 def bench_plan(name):
     """The plan of one benchmarked workload, at the batch and precision bench.py runs it: the EDM nets in fp16f8 (FFHQ with f8 only
     in blocks of >= 256 channels), the SD-1.5 eps-net at batch 8 under classifier-free guidance (16 contexts), its VAE decoder."""
+    return bench_plan_weights(name, dezero=False)[0]
+
+
+def bench_plan_weights(name, batch=None, dezero=True):
+    """bench_plan with its weights: (plan, weight blob bytes, model config).  batch replaces the benchmark batch (EDM nets: images;
+    SD-1.5: prompts, run under guidance as 2 x batch; VAE: latents).  dezero gives the EDM nets the weight set bench.py runs, with
+    seeded per-channel GroupNorm gains and biases (the init's are ones and zeros, which would hide a coefficient applied to the
+    wrong channel of its group)."""
     from diff_sampler_b200 import gemm_replay
     if name in ('cifar10', 'ffhq', 'imagenet64'):
-        return gemm_replay.edm_plan(name, {'cifar10': 512}.get(name, 256), 256 if name == 'ffhq' else 0)
+        from diff_sampler_b200 import edm_nets
+        B = batch or {'cifar10': 512}.get(name, 256)
+        pl, wb = gemm_replay.edm_plan(name, B, 256 if name == 'ffhq' else 0, dezero=dezero, norm_jitter=dezero, with_weights=True)
+        return pl, wb, edm_nets.NET_CONFIGS[name]
     if name == 'sd15':
         from diff_sampler_b200 import ldm_plan
         from oracle import ldm_oracle as LO
         P, cfg = LO.make_params('sd15')
         st = ldm_plan.ldm_structure(P, cfg['num_heads'])
         wb, info = ldm_plan.pack_ldm_weights(st, P, f8=True, f8_linear=True)
-        return ldm_plan.compile_ldm_plan(st, wb, info, 8, 16, 1, cfg['img_resolution'], npass=3, f8=True, f8_linear=True)
+        B = batch or 8
+        pl = ldm_plan.compile_ldm_plan(st, wb, info, B, 2 * B, 1, cfg['img_resolution'], npass=3, f8=True, f8_linear=True)
+        return pl, wb.bytes(), cfg
     from diff_sampler_b200 import vae_plan
     from oracle import vae_oracle as VO
     P, cfg = VO.make_params('sd_vae', seed=0)
     mods, meta = vae_plan.vae_structure(P)
-    return vae_plan.compile_vae_plan(mods, meta, vae_plan.pack_vae_weights(mods, meta, P), 1, 64)
+    wb = vae_plan.pack_vae_weights(mods, meta, P)
+    return vae_plan.compile_vae_plan(mods, meta, wb, batch or 1, 64), wb.bytes(), dict(cfg, **meta)
 
 
 def replay_key(cfg):
@@ -354,7 +368,8 @@ def test_coverage_table(sms):
     for r in TABLE:
         print(_fmt(r))
     print('rows-mode replays lay the operands out z-major: the head windows of the plans\' attention products (a_c_per_zh, '
-          'b_k_per_zh, b_row_per_zh, b_k0) are not reproduced; test_gpu_kernels.py covers them at the BN fill_bn picks')
+          'b_k_per_zh, b_row_per_zh, b_k0) are not reproduced; test_gpu_kernels.py covers them at the BN fill_bn picks, and '
+          'test_gpu_plan_ops.py runs the plans\' own descriptors')
     # each assertion covers what ran (a -k selection may keep only some launches)
     sweep = [r for r in TABLE if r['kind'].startswith('sweep')]
     plan = [r for r in TABLE if r['kind'].startswith('plan')]

@@ -505,7 +505,14 @@ def test_fused_attention_causal(lib, B, nh, L, d):
     _fused_attention(lib, B, nh, L, L, d, causal=True)
 
 
-def _fused_attention(lib, B, nh, L, Lk, d, causal):
+def test_fused_attention_long_keys(lib):
+    """4096 keys (the SD-1.5 64x64 self-attention, 40-wide heads) with values of non-zero mean: the P V product adds up over the
+    whole key range.  Accumulated in one wgmma accumulator its fp32 error grew linearly with the key count and reached 3.4e-5 of
+    max |out| on the plan's own activations; each 64-key block now has its own accumulator."""
+    _fused_attention(lib, 2, 2, 4096, 4096, 40, causal=False, v_mean=1.0)
+
+
+def _fused_attention(lib, B, nh, L, Lk, d, causal, v_mean=0.0):
     """attn_kernel (QK^T -> online softmax -> PV in one kernel, head dim padded to 64) against float64 softmax attention on the
     same fp16 hi+lo operands: self-attention shapes, a cross-attention shape (77 keys, pitch 80), partial query / key tiles."""
     from diff_sampler_b200 import _cstructs as S
@@ -513,7 +520,7 @@ def _fused_attention(lib, B, nh, L, Lk, d, causal):
     hp = nh * 64
     q = torch.randn(B, nh, L, d, device=dev()) * 1.5
     k = torch.randn(B, nh, Lk, d, device=dev()) * 1.5
-    v = torch.randn(B, nh, Lk, d, device=dev())
+    v = torch.randn(B, nh, Lk, d, device=dev()) + v_mean
     k[:, :, 3] *= 4.0                                    # a dominant key: peaky rows
     scale = d ** -0.5
     qk = torch.zeros(B, max(L, Lk), 2 * hp, device=dev())

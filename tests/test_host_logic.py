@@ -407,3 +407,108 @@ def test_benchmark_plans_cover_the_gemm_tile_configurations():
     assert any(c.edm == 1 for c in cfgs)
     assert any(c.mode == 'rows' for c in cfgs)
     assert any(c.f8 and c.BN in (192, 256) for c in cfgs)
+
+
+def _tiny_plans():
+    """(name, plan, weight bytes, io) of every plan kind, at the sizes tests/test_plan_interp.py runs them."""
+    from diff_sampler_b200 import clip_plan, ldm_plan, vae_plan
+    from oracle import clip_oracle as CO, ldm_oracle as LO, vae_oracle as VO
+    for name, f8 in (('tiny_song', False), ('tiny_adm', False), ('tiny_song', True), ('tiny_adm', True)):
+        P, St = O.make_net(name, seed=0, dezero=True)
+        spec = edm_nets.spec_from_params(P, St['img_resolution'], St['img_channels'], St['label_dim'])
+        spec.sigma_data = 0.5
+        wb, info = planner.pack_weights(spec, P, f8=f8)
+        B, R = 3, St['img_resolution']
+        pl = planner.compile_plan(spec, wb, info, B, 1, B if spec.label_dim else 0, npass=3, f8=f8)
+        lab = torch.eye(spec.label_dim)[torch.arange(B) % spec.label_dim].contiguous() if spec.label_dim else None
+        yield (f'{name} f8={f8}', pl, wb.bytes(), {S.DS_IO_X: O.stacked_randn(range(B), (3, R, R)) * 2.0, S.DS_IO_D: torch.zeros(B, 3, R, R),
+                                                  S.DS_IO_SIGMA: torch.tensor([2.0]), S.DS_IO_LABELS: lab, S.DS_IO_BOTTLENECK: torch.zeros(B, 64)})
+    P, cfg = LO.make_params('tiny_ldm')
+    st = ldm_plan.ldm_structure(P, cfg['num_heads'])
+    for mode in ('fp16x3', 'f8', 'f8_linear'):
+        f8, f8l = mode != 'fp16x3', mode == 'f8_linear'
+        wb, info = ldm_plan.pack_ldm_weights(st, P, f8=f8, f8_linear=f8l)
+        B, Bt, R, C = 2, 4, cfg['img_resolution'], cfg['in_channels']
+        pl = ldm_plan.compile_ldm_plan(st, wb, info, B, Bt, 1, R, npass=3, f8=f8, f8_linear=f8l)
+        g = torch.Generator().manual_seed(5)
+        yield (f'tiny_ldm {mode}', pl, wb.bytes(), {S.DS_IO_X: torch.randn(B, C, R, R, generator=g), S.DS_IO_D: torch.zeros(Bt, C, R, R),
+                                                    S.DS_IO_SIGMA: torch.tensor([417.0]), S.DS_IO_LABELS: torch.tensor([[0.0, 0.0, 0.37, 0.0]]),
+                                                    S.DS_IO_BOTTLENECK: torch.zeros(Bt, 64),
+                                                    S.DS_IO_CTX: torch.randn(Bt, 77, cfg['context_dim'], generator=g)})
+    P, cfg = VO.make_params('tiny_vae', seed=0)
+    mods, meta = vae_plan.vae_structure(P)
+    wb = vae_plan.pack_vae_weights(mods, meta, P)
+    pl = vae_plan.compile_vae_plan(mods, meta, wb, 2, 8)
+    z = torch.randn(2, cfg['z_channels'], 8, 8, generator=torch.Generator().manual_seed(3)) * cfg['scale_factor'] * 1.3
+    yield ('tiny_vae', pl, wb.bytes(), {S.DS_IO_X: z, S.DS_IO_D: torch.zeros(2, meta['out_ch'], 8 * meta['upscale'], 8 * meta['upscale']),
+                                        S.DS_IO_LABELS: torch.tensor([[0.0, 0.0, 1.0 / cfg['scale_factor'], 0.0]])})
+    P, cfg = CO.make_params('tiny_clip', seed=0)
+    ccfg = clip_plan.clip_config(P)
+    wb = clip_plan.pack_clip_weights(P, ccfg)
+    ids = torch.randint(0, cfg['vocab_size'], (2, 77), generator=torch.Generator().manual_seed(4)).to(torch.int32)
+    pl = clip_plan.compile_clip_plan(ccfg, wb, 2, 77)
+    yield ('tiny_clip', pl, wb.bytes(), {S.DS_IO_X: ids, S.DS_IO_D: torch.zeros(2, 77, cfg['hidden_size'])})
+
+
+def test_plan_op_write_spans_cover_every_store_of_the_interpreter():
+    """tests/plan_spans.writes() is the span table the GPU op replay (tests/test_gpu_plan_ops.py) fills with NaN and outside of which
+    it demands the arena unchanged byte for byte.  Here every op of every plan kind runs on the CPU interpreter, and every byte it
+    changes -- arena and io slots -- must lie inside the op's spans; every pointer field must resolve."""
+    from oracle import plan_interp as PI
+    from plan_spans import resolve, writes
+    seen = set()
+    for name, pl, wb, io in _tiny_plans():
+        io = {k: (v.contiguous() if v is not None else None) for k, v in io.items()}
+        mem = PI.Memory(pl.arena_bytes, wb, io)
+        regions = {S.SPACE_ARENA: mem.arena}
+        regions.update({(S.SPACE_IO, k): v.reshape(-1).view(torch.uint8) for k, v in io.items() if v is not None})
+        for i in range(pl.n_ops):
+            op = pl.ops_array[i]
+            seen.add(op.type)
+            resolve(op, mem.arena, mem.weights, io)
+            before = {k: r.clone() for k, r in regions.items()}
+            PI.run_op(mem, op)
+            inside = {k: torch.zeros(r.numel(), dtype=torch.bool) for k, r in regions.items()}
+            for s in writes(op):
+                space, off = s.ref >> 60, s.ref & PI.MASK60
+                key = space if space == S.SPACE_ARENA else (space, off)
+                if key not in inside:
+                    continue
+                o = off if space == S.SPACE_ARENA else 0
+                assert o + s.nbytes <= inside[key].numel(), (name, i, s)
+                inside[key][o:o + s.nbytes] = True
+            for k, r in regions.items():
+                stray = (r != before[k]) & ~inside[k]
+                assert not stray.any(), (name, i, S.UNION_FIELD[op.type], op.tag, k, stray.nonzero()[:4].reshape(-1).tolist())
+    assert seen == set(S.UNION_FIELD), sorted(S.UNION_FIELD[t] for t in set(S.UNION_FIELD) - seen)
+
+
+def test_plan_op_spans_and_resolve_handle_the_benchmarked_plans():
+    """Every op type of the five benchmarked plans (host-compiled, as tests/test_gpu_gemm_tiles.bench_plan builds them) has a span
+    table entry and resolves."""
+    from plan_spans import resolve, writes
+    from test_gpu_gemm_tiles import WORKLOADS, bench_plan
+    class Buf:                                   # stands in for a device buffer: resolve() only needs a base address and a size
+        def __init__(self, base, n):
+            self.base, self.n = base, n
+
+        def data_ptr(self):
+            return self.base
+
+        def numel(self):
+            return self.n
+    for name in WORKLOADS:
+        pl = bench_plan(name)
+        types = set()
+        for i in range(pl.n_ops):
+            op = pl.ops_array[i]
+            types.add(S.UNION_FIELD[op.type])
+            resolve(op, Buf(1 << 40, pl.arena_bytes), Buf(1 << 44, 1 << 40), {k: Buf((k + 1) << 32, 1) for k in range(6)})
+            spans = writes(op)
+            assert spans or op.type == S.DS_OP_CHANMEAN, (name, i)
+            assert all(s.nbytes > 0 and s.ref >> 60 in (S.SPACE_ARENA, S.SPACE_IO) for s in spans), (name, i, spans)
+            for s in spans:
+                if s.ref >> 60 == S.SPACE_ARENA:
+                    assert (s.ref & ((1 << 60) - 1)) + s.nbytes <= pl.arena_bytes, (name, i, s)
+        print(name, pl.n_ops, sorted(types))
+        assert {'gemm', 'gn_apply', 'memset'} <= types
