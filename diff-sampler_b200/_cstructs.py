@@ -9,7 +9,7 @@ F32 = C.c_float
 
 DS_OP_GEMM, DS_OP_GN_STATS, DS_OP_GN_APPLY, DS_OP_SOFTMAX, DS_OP_POSEMB, DS_OP_LINEAR = 1, 2, 3, 4, 5, 6
 DS_OP_PREP_INPUT, DS_OP_CHANMEAN, DS_OP_MEMSET, DS_OP_LAYERNORM, DS_OP_GEGLU, DS_OP_GN_FINALIZE, DS_OP_ATTN, DS_OP_EMBED = 7, 8, 9, 10, 11, 12, 13, 14
-DS_IO_X, DS_IO_D, DS_IO_SIGMA, DS_IO_LABELS, DS_IO_BOTTLENECK, DS_IO_CTX = 0, 1, 2, 3, 4, 5
+DS_IO_X, DS_IO_D, DS_IO_SIGMA, DS_IO_LABELS, DS_IO_BOTTLENECK, DS_IO_CTX, DS_IO_COUNT = 0, 1, 2, 3, 4, 5, 6
 DS_M_X0, DS_M_EPS, DS_M_DIV, DS_M_NONE = 0, 1, 2, 3
 DS_F8_SH_A16, DS_F8_SH_LO8, DS_F8_SH_HI8 = 6, 13, 2      # csrc/ops.h: power-of-two operand scales of the f8 GEMM mode
 

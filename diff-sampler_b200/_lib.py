@@ -3,6 +3,8 @@ missing or a call fails, this raises."""
 import ctypes as C
 import os
 
+import torch
+
 from . import _cstructs as S
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -89,3 +91,55 @@ def gemm_config(desc):
     info = (C.c_int * 2)()
     check(load().ds_gemm_config(C.byref(desc), info), 'ds_gemm_config')
     return dict(stages=info[0], grid=info[1])
+
+
+class NativePlans:
+    """One weight blob on a CUDA device (ds_weights_create) and the native plans compiled against it (ds_unet_create), keyed by the
+    shape they were compiled for.  Destroys every handle when collected."""
+
+    def __init__(self, blob, device):
+        self.lib = load()
+        self.device = device
+        self.plans = {}                 # key -> (ds_unet handle, plan.Plan)
+        self._wh = C.c_void_p()
+        with torch.cuda.device(device):
+            check(self.lib.ds_weights_create(blob, len(blob), C.byref(self._wh)), 'ds_weights_create')
+
+    def get(self, key, compile_fn, io_bytes=None):
+        """(handle, plan) for `key`; the plan is compile_fn() on first use.  io_bytes(plan) -> the byte sizes of the six io slots turns
+        on CUDA-graph replay of every forward (ds_unet_enable_graph)."""
+        ent = self.plans.get(key)
+        if ent is None:
+            pl = compile_fn()
+            h = C.c_void_p()
+            with torch.cuda.device(self.device):
+                check(self.lib.ds_unet_create(self._wh, C.cast(pl.ops_array, C.c_void_p), pl.n_ops, C.sizeof(S.PlanOp), pl.arena_bytes,
+                                              C.byref(h)), 'ds_unet_create')
+                if io_bytes is not None:
+                    check(self.lib.ds_unet_enable_graph(h, (C.c_size_t * S.DS_IO_COUNT)(*io_bytes(pl)), S.DS_IO_COUNT),
+                          'ds_unet_enable_graph')
+            ent = self.plans[key] = (h, pl)
+        return ent
+
+    def run(self, h, io, stream):
+        """One forward of plan handle h over the io slots (device pointers or None, DS_IO_* order) on `stream`.
+        Returns the number of kernels it launched."""
+        check(self.lib.ds_unet_forward_io(h, (C.c_void_p * S.DS_IO_COUNT)(*io), S.DS_IO_COUNT, C.c_void_p(stream)), 'ds_unet_forward_io')
+        return self.lib.ds_unet_last_launch_count(h)
+
+    def debug_read(self, key, name, numel, dtype=torch.float32):
+        """Copy the arena buffer `name` of the plan for `key` to the host (tests only)."""
+        h, pl = self.plans[key]
+        t = torch.empty(numel, dtype=dtype)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        check(self.lib.ds_unet_debug_read(h, pl.arena_offsets[name], t.data_ptr(), t.numel() * t.element_size(), C.c_void_p(stream)),
+              'ds_unet_debug_read')
+        return t
+
+    def __del__(self):
+        try:
+            for h, _ in self.plans.values():
+                self.lib.ds_unet_destroy(h)
+            self.lib.ds_weights_destroy(self._wh)
+        except Exception:
+            pass

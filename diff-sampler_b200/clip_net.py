@@ -9,12 +9,10 @@ models/ldm/modules/encoders/modules.py:137-159 `FrozenCLIPEmbedder`): token ids 
 Tokenisation stays with the reference's own `CLIPTokenizer` object (a vocabulary lookup on the host); everything after it runs as one
 plan on the GPU (clip_plan.py).  No CPU fallback.
 """
-import ctypes as C
 from collections import OrderedDict
 
 import torch
 
-from . import _cstructs as S
 from . import _lib
 from . import clip_plan
 
@@ -31,11 +29,7 @@ class B200CLIPTextEncoder:
         self.tokenizer = tokenizer
         self.max_length = int(max_length)
         self.wb = clip_plan.pack_clip_weights(params, self.cfg)
-        blob = self.wb.bytes()
-        self._wh = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.ds_weights_create(blob, len(blob), C.byref(self._wh)), 'ds_weights_create')
-        self._plans = {}
+        self.native = _lib.NativePlans(self.wb.bytes(), self.device)
         self.total_launches = 0
 
     @classmethod
@@ -55,16 +49,7 @@ class B200CLIPTextEncoder:
         return cls(sd, **kw)
 
     def _plan(self, B, T):
-        ent = self._plans.get((B, T))
-        if ent is None:
-            pl = clip_plan.compile_clip_plan(self.cfg, self.wb, B, T, num_heads=self.num_heads, eps=self.eps)
-            h = C.c_void_p()
-            with torch.cuda.device(self.device):
-                _lib.check(self.lib.ds_unet_create(self._wh, C.cast(pl.ops_array, C.c_void_p), pl.n_ops, C.sizeof(S.PlanOp), pl.arena_bytes,
-                                                   C.byref(h)), 'ds_unet_create')
-            ent = (h, pl)
-            self._plans[(B, T)] = ent
-        return ent
+        return self.native.get((B, T), lambda: clip_plan.compile_clip_plan(self.cfg, self.wb, B, T, num_heads=self.num_heads, eps=self.eps))
 
     def __call__(self, tokens, out=None):
         """tokens: integer tensor [B, T] on the CUDA device -> last_hidden_state [B, T, hidden] fp32.  A str / list of str is tokenised
@@ -80,10 +65,8 @@ class B200CLIPTextEncoder:
         h, pl = self._plan(B, T)
         if out is None:
             out = torch.empty(B, T, self.cfg['hidden_size'], device=ids.device, dtype=torch.float32)
-        io = (C.c_void_p * 6)(ids.data_ptr(), out.data_ptr(), None, None, None, None)
-        stream = torch.cuda.current_stream(ids.device).cuda_stream
-        _lib.check(self.lib.ds_unet_forward_io(h, io, 6, C.c_void_p(stream)), 'ds_unet_forward_io')
-        self.total_launches += self.lib.ds_unet_last_launch_count(h)
+        self.total_launches += self.native.run(h, (ids.data_ptr(), out.data_ptr(), None, None, None, None),
+                                               torch.cuda.current_stream(ids.device).cuda_stream)
         return out
 
     forward = __call__
@@ -97,17 +80,5 @@ class B200CLIPTextEncoder:
         return self(enc['input_ids'].to(self.device))
 
     def debug_read(self, B, T, name, numel, dtype=torch.float32):
-        h, pl = self._plan(B, T)
-        t = torch.empty(numel, dtype=dtype)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(self.lib.ds_unet_debug_read(h, pl.arena_offsets[name], t.data_ptr(), t.numel() * t.element_size(), C.c_void_p(stream)),
-                   'ds_unet_debug_read')
-        return t
-
-    def __del__(self):
-        try:
-            for h, _ in self._plans.values():
-                self.lib.ds_unet_destroy(h)
-            self.lib.ds_weights_destroy(self._wh)
-        except Exception:
-            pass
+        self._plan(B, T)
+        return self.native.debug_read((B, T), name, numel, dtype)

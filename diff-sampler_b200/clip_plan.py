@@ -16,15 +16,9 @@ import torch
 
 from . import _cstructs as S
 from . import gemm_desc as G
-from .plan import Plan, WeightBlob, _Arena
+from .plan import F4, H2, NPL, PlanBuilder, WeightBlob, io
 
-F4, H2 = 4, 2
 KEYS_PITCH = 128              # V^T row pitch (keys per row; a multiple of 8 elements for the TMA strides)
-
-
-def prows(n):
-    bn, tiles = G.pick_bn(n)
-    return bn * tiles
 
 
 def clip_config(params):
@@ -43,26 +37,21 @@ def pack_clip_weights(params, cfg):
     H = cfg['hidden_size']
     assert H % 64 == 0 and cfg['intermediate_size'] % 64 == 0
 
-    def lin(key, w, b):
-        wb.add(key + ':w', G.pack_conv_weight(w.reshape(w.shape[0], w.shape[1], 1, 1)))
-        wb.add(key + ':b', b)
-
     wb.add('tok', P('text_model.embeddings.token_embedding.weight'))
     wb.add('pos', P('text_model.embeddings.position_embedding.weight'))
     for i in range(cfg['num_hidden_layers']):
         p = f'text_model.encoder.layers.{i}.'
         a = p + 'self_attn.'
-        lin(f'l{i}.qk', torch.cat([P(a + 'q_proj.weight'), P(a + 'k_proj.weight')]), torch.cat([P(a + 'q_proj.bias'), P(a + 'k_proj.bias')]))
+        wb.add_gemm(f'l{i}.qk', torch.cat([P(a + 'q_proj.weight'), P(a + 'k_proj.weight')]),
+                    bias=torch.cat([P(a + 'q_proj.bias'), P(a + 'k_proj.bias')]))
         wb.add(f'l{i}.v:w', G.split_planes(P(a + 'v_proj.weight')))          # A operand of the V^T product: rows unpadded
         wb.add(f'l{i}.v:b', P(a + 'v_proj.bias'))
-        lin(f'l{i}.out', P(a + 'out_proj.weight'), P(a + 'out_proj.bias'))
-        lin(f'l{i}.fc1', P(p + 'mlp.fc1.weight'), P(p + 'mlp.fc1.bias'))
-        lin(f'l{i}.fc2', P(p + 'mlp.fc2.weight'), P(p + 'mlp.fc2.bias'))
+        wb.add_gemm(f'l{i}.out', P(a + 'out_proj.weight'), bias=P(a + 'out_proj.bias'))
+        wb.add_gemm(f'l{i}.fc1', P(p + 'mlp.fc1.weight'), bias=P(p + 'mlp.fc1.bias'))
+        wb.add_gemm(f'l{i}.fc2', P(p + 'mlp.fc2.weight'), bias=P(p + 'mlp.fc2.bias'))
         for k in ('layer_norm1', 'layer_norm2'):
-            wb.add(f'l{i}.{k}:g', P(p + k + '.weight'))
-            wb.add(f'l{i}.{k}:b', P(p + k + '.bias'))
-    wb.add('final:g', P('text_model.final_layer_norm.weight'))
-    wb.add('final:b', P('text_model.final_layer_norm.bias'))
+            wb.add_norm(f'l{i}.{k}', P, p + k)
+    wb.add_norm('final', P, 'text_model.final_layer_norm')
     return wb
 
 
@@ -75,27 +64,23 @@ def compile_clip_plan(cfg, wb, B, T, num_heads=None, eps=1e-5, npass=3):
     if T > cfg['max_position_embeddings'] or T > KEYS_PITCH:
         raise ValueError(f'{T} tokens exceed the position table ({cfg["max_position_embeddings"]})')
     M = B * T
-    npl = 2
-    A = _Arena()
-    ops = []
-    emit = ops.append
-    io = lambda slot: S.ref(S.SPACE_IO, slot)
-    W = wb.ref
-    A.need('h0', M * H * F4)
-    A.need('h1', M * H * F4)
-    A.need('ln', npl * M * H * H2)
-    A.need('qk', npl * M * 2 * H * H2)
-    A.need('vt', npl * B * H * KEYS_PITCH * H2)
-    A.need('o', npl * M * H * H2)
-    A.need('ff', M * I * F4)
-    A.need('gg', npl * M * I * H2)
+    pb = PlanBuilder(wb, B, npass, tag=None)           # each op tagged with its index
+    emit, W = pb.emit, wb.ref
+    pb.need('h0', M * H * F4)
+    pb.need('h1', M * H * F4)
+    pb.need('ln', NPL * M * H * H2)
+    pb.need('qk', NPL * M * 2 * H * H2)
+    pb.need('vt', NPL * B * H * KEYS_PITCH * H2)
+    pb.need('o', NPL * M * H * H2)
+    pb.need('ff', M * I * F4)
+    pb.need('gg', NPL * M * I * H2)
 
     def layernorm(src, g, b, out, fmt=0):
-        emit(lambda R_: S.LayernormDesc(src=R_(src), gamma=W(g), beta=W(b), out=out(R_), rows=M, C=H, nplanes=npl, eps=eps, fmt=fmt))
+        emit(lambda R_: S.LayernormDesc(src=R_(src), gamma=W(g), beta=W(b), out=out(R_), rows=M, C=H, nplanes=NPL, eps=eps, fmt=fmt))
 
     def linear(a, K, key, N, **kw):
         """[M][K] activation planes x packed weight [N][K] (+ bias[N]) through the batched-rows GEMM form."""
-        emit(lambda R_: G.rows_gemm(R_(a), M, K, 1, W(key + ':w'), prows(N), K, 1, K, num_z=1, nh=1, m_valid=M, n_valid=N, npass=npass,
+        emit(lambda R_: G.rows_gemm(R_(a), M, K, 1, W(key + ':w'), G.padded_rows(N), K, 1, K, num_z=1, nh=1, m_valid=M, n_valid=N, npass=npass,
                                     bias_n=W(key + ':b'), ldo=N, **{k: (v(R_) if callable(v) else v) for k, v in kw.items()})[0])
 
     emit(lambda R_: S.EmbedDesc(ids=io(S.DS_IO_X), tok=W('tok'), pos=W('pos'), out=R_('h0'), rows=M, T=T, C=H, vocab=cfg['vocab_size']))
@@ -104,26 +89,14 @@ def compile_clip_plan(cfg, wb, B, T, num_heads=None, eps=1e-5, npass=3):
         # ---- h1 = h0 + out_proj(causal_attention(LN1(h0)))
         layernorm('h0', L + '.layer_norm1:g', L + '.layer_norm1:b', lambda R_: R_('ln'))
         linear('ln', H, L + '.qk', 2 * H, out_h16=lambda R_: R_('qk'), o_plane=M * 2 * H)
-        # V^T[b][c][key] = sum_k Wv[c][k] LN[b][key][k] + bv[c]: written transposed, the layout the P.V product reads
-        emit(lambda R_, L=L: G.rows_gemm(W(L + '.v:w'), H, H, 1, R_('ln'), T, H, B, H, num_z=B, nh=1, m_valid=H, n_valid=T, npass=npass,
-                                         b_z_per_zb=1, bias_m=W(L + '.v:b'), out_h16=R_('vt'), o_zb=H * KEYS_PITCH, ldo=KEYS_PITCH,
-                                         o_plane=B * H * KEYS_PITCH)[0])
-        emit(lambda R_: S.AttnDesc(q=R_('qk'), k=R_('qk'), vt=R_('vt'), out=R_('o'), B=B, nh=nh, L=T, Lk=T, q_pitch=2 * H, q_c0=0, k_pitch=2 * H,
-                                   k_c0=H, vt_pitch=KEYS_PITCH, o_pitch=H, nplanes=npl, scale=64 ** -0.5, causal=1))
+        pb.vt_gemm(L + '.v:w', 'ln', H, H, T, KEYS_PITCH, bias=L + '.v:b')
+        pb.attention(True, 'qk', 'qk', 'o', nh, T, T, 64, 64 ** -0.5, KEYS_PITCH, causal=1)
         linear('o', H, L + '.out', H, out_f32=lambda R_: R_('h1'), residual=lambda R_: R_('h0'), ldr=H)
         # ---- h0 = h1 + fc2(quick_gelu(fc1(LN2(h1))))
         layernorm('h1', L + '.layer_norm2:g', L + '.layer_norm2:b', lambda R_: R_('ln'))
         linear('ln', H, L + '.fc1', I, out_f32=lambda R_: R_('ff'))
-        emit(lambda R_: S.GegluDesc(src=R_('ff'), out=R_('gg'), rows=M, I=I, nplanes=npl, fmt=0, mode=1))
+        emit(lambda R_: S.GegluDesc(src=R_('ff'), out=R_('gg'), rows=M, I=I, nplanes=NPL, fmt=0, mode=1))
         linear('gg', I, L + '.fc2', H, out_f32=lambda R_: R_('h0'), residual=lambda R_: R_('h1'), ldr=H)
     layernorm('h0', 'final:g', 'final:b', lambda R_: io(S.DS_IO_D), fmt=2)
 
-    total = A.finalize()
-    arr = (S.PlanOp * len(ops))()
-    for i, builder in enumerate(ops):
-        desc = builder(A.ref)
-        arr[i].type = S.OP_TYPE_OF[type(desc)]
-        arr[i].tag = i
-        setattr(arr[i].u, S.UNION_FIELD[arr[i].type], desc)
-    meta = dict(B=B, T=T, npass=npass, n_ops=len(ops), n_gemm=sum(1 for i in range(len(ops)) if arr[i].type == S.DS_OP_GEMM))
-    return Plan(arr, len(ops), total, dict(A.offsets), meta)
+    return pb.finish(B=B, T=T, npass=npass)

@@ -50,6 +50,12 @@ def fill_bn(n, m_tiles, num_z=1):
     return best[1], best[2]
 
 
+def padded_rows(n):
+    """Row count of a weight packed by pack_conv_weight / pack_conv_weight_f8: pick_bn's whole N tiles."""
+    bn, tiles = pick_bn(n)
+    return bn * tiles
+
+
 def split_planes_rows(n_valid, bn):
     tiles = -(-n_valid // bn)
     return tiles, tiles * bn
@@ -71,10 +77,11 @@ def conv_box(H, W):
 
 def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w_planes=2, a2_ptr=0, C2=0,
               out_f32=0, out_h16=0, o_planes=2, ldo=None, bias=0, rowvec=0, rowvec_stride=0, residual=0, ldr=None, scale=1.0,
-              edm=None, bn=None, s2d=False, f8=False, acc_scale=1.0):
+              edm=None, nchw_out=None, bn=None, s2d=False, f8=False, acc_scale=1.0):
     """3x3 (taps=9) or 1x1 (taps=1) convolution over NHWC fp16 planes [a_planes][Bn][H][W][C] with the
     packed weight matrix [w_planes][Cout_pad][taps*C + C2] (K ordered tap-major, then the aux/skip block).
     Output rows are NHWC pixels: out[pixel][cout] (+ fused epilogue).
+    edm = (x, coef, coef_stride, C, D): D = c_skip x + c_out y as NCHW fp32 (the EDM combine); nchw_out = (C, D): y as NCHW fp32.
     f8=True: both operands are in the fp16 + 2 x e4m3 layout of csrc/ops.h (activations from ds_gn_apply fmt=1, weights from
     pack_conv_weight_f8); acc_scale = 2^-S of that packed weight."""
     assert C % 64 == 0 and C2 % 64 == 0
@@ -86,8 +93,7 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     d = S.GemmDesc()
     bw, bh, bnn = conv_box(H, W)
     BN, n_tiles = (bn, -(-Cout // bn)) if bn else fill_bn(Cout, -(-(Bn * H * W) // 128))
-    pbn, ptiles = pick_bn(Cout)
-    cout_pad = pbn * ptiles              # rows of the packed weight (pack_conv_weight); tiles past it read TMA zero fill
+    cout_pad = padded_rows(Cout)         # rows of the packed weight; tiles past it read TMA zero fill
     ktot = taps * C + C2
     d.a_ptr = a_ptr
     cphys = 4 * C if s2d else C          # physical channel extent of the activation tensor
@@ -140,6 +146,9 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     if edm is not None:
         d.edm_out = 1
         d.edm_x, d.edm_coef, d.edm_coef_stride, d.edm_C, d.edm_D = edm
+    if nchw_out is not None:
+        d.edm_out = 2
+        d.edm_C, d.edm_D = nchw_out
     return d, dict(BN=BN, n_tiles=n_tiles, cout_pad=cout_pad, ktot=ktot)
 
 

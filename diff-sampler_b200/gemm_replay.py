@@ -170,19 +170,20 @@ def make_desc(cfg, dev, bn=None, batch=None, pad=False, seed=0):
             bufs['a'] = G.split_planes(bufs['x'])
             if C2:
                 bufs['a2'] = G.split_planes(bufs['x2'])
-        edm = None
+        edm = nchw_out = None
         if cfg.edm:
             bufs['edm_x'] = rnd(Bn, N, H, W).to(dev)
             bufs['edm_coef'] = (torch.rand(Bn, 4, generator=g) + 0.5).to(dev)
             bufs['D'] = fill((Bn * N * H * W + (64 if pad else 0),))
-            edm = (ptr('edm_x'), ptr('edm_coef'), 4, N, ptr('D'))
+            if cfg.edm == 2:
+                nchw_out = (N, ptr('D'))
+            else:
+                edm = (ptr('edm_x'), ptr('edm_coef'), 4, N, ptr('D'))
         d, info = G.conv_gemm(ptr('a'), Bn, H, W, C, ptr('wp'), N, taps=cfg.taps, npass=cfg.npass, a2_ptr=ptr('a2'), C2=C2,
                               out_f32=ptr('out'), out_h16=ptr('outh'), o_planes=2 if cfg.planes else 1, ldo=ldo, bias=ptr('bias_n'),
                               rowvec=ptr('rowvec'), rowvec_stride=N if cfg.rowvec == 2 else 0, residual=ptr('residual'), ldr=N,
-                              scale=scale, edm=edm, bn=BN, s2d=cfg.s2d, f8=cfg.f8, acc_scale=acc)
+                              scale=scale, edm=edm, nchw_out=nchw_out, bn=BN, s2d=cfg.s2d, f8=cfg.f8, acc_scale=acc)
         d.bias_m = ptr('bias_m')
-        if cfg.edm == 2:
-            d.edm_out = 2
         d.o_plane = rows_out * ldo if cfg.planes else 0
     else:
         assert not cfg.rowvec and not cfg.f8 and not cfg.edm, 'rows mode has no conditioning rows, f8 passes or image store'

@@ -6,7 +6,6 @@ sigma_min, sigma_max, sigma(), sigma_inv(), round_sigma()).  The eps-net runs in
 the sigma <-> t interpolation over the 1000 log-alpha knots is a few scalar torch ops on the device.
 """
 import ctypes as C
-import math
 from collections import OrderedDict
 
 import torch
@@ -14,9 +13,8 @@ import torch
 from . import _cstructs as S
 from . import _lib
 from . import ldm_plan
+from .net import PRECISIONS, default_cuda_graph, default_precision
 from .solver_utils import solver_update
-
-PRECISIONS = {'fp16x3': 3, 'fp16': 1, 'fp16f8': 3}       # fp16f8: ResBlock convolutions in the f8 GEMM mode (net.py, csrc/ops.h)
 
 
 def make_alphas_cumprod(linear_start=0.00085, linear_end=0.0120, n=1000):
@@ -34,12 +32,9 @@ class B200LDMNet:
         self.lib = _lib.load()
         self.img_resolution, self.img_channels, self.label_dim = img_resolution, img_channels, True
         self.guidance_type, self.guidance_rate = guidance_type, guidance_rate
-        if precision is None:
-            from .net import default_precision
-            precision = default_precision()
-        self.precision = precision
-        self.npass = PRECISIONS[precision]
-        self.f8 = precision == 'fp16f8'
+        self.precision = precision or default_precision()
+        self.npass = PRECISIONS[self.precision]
+        self.f8 = self.precision == 'fp16f8'           # ResBlock convolutions in the f8 GEMM mode (csrc/ops.h)
         # with fp16f8, proj_in / attn2.to_q / GEGLU ff / proj_out also run in the f8 GEMM mode (held by the f8 parity tests;
         # DSB_LDM_F8_LINEAR=0 or f8_linear=False keeps them fp16x3)
         if f8_linear is None:
@@ -47,17 +42,10 @@ class B200LDMNet:
             f8_linear = os.environ.get('DSB_LDM_F8_LINEAR', '1') != '0'
         self.f8_linear = bool(f8_linear) and self.f8
         self.flash_attn = bool(flash_attn)
-        if cuda_graph is None:
-            from .net import default_cuda_graph
-            cuda_graph = default_cuda_graph()
-        self.cuda_graph = bool(cuda_graph)
+        self.cuda_graph = default_cuda_graph() if cuda_graph is None else bool(cuda_graph)
         self.st = ldm_plan.ldm_structure(params, num_heads)
         self.wb, self.info = ldm_plan.pack_ldm_weights(self.st, params, f8=self.f8, f8_linear=self.f8_linear)
-        blob = self.wb.bytes()
-        self._wh = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.ds_weights_create(blob, len(blob), C.byref(self._wh)), 'ds_weights_create')
-        self._plans = {}
+        self.native = _lib.NativePlans(self.wb.bytes(), self.device)
         self.total_launches = 0
         ac = make_alphas_cumprod() if alphas_cumprod is None else torch.as_tensor(alphas_cumprod).float()
         log_alphas = 0.5 * torch.log(ac)
@@ -111,23 +99,12 @@ class B200LDMNet:
 
     # ---- plan cache ---------------------------------------------------------------------------------------------------------
     def _plan(self, B, Bt, nT):
-        key = (B, Bt, nT)
-        ent = self._plans.get(key)
-        if ent is None:
-            pl = ldm_plan.compile_ldm_plan(self.st, self.wb, self.info, B, Bt, nT, self.img_resolution, npass=self.npass,
-                                               flash_attn=self.flash_attn, f8=self.f8, f8_linear=self.f8_linear)
-            h = C.c_void_p()
-            with torch.cuda.device(self.device):
-                _lib.check(self.lib.ds_unet_create(self._wh, C.cast(pl.ops_array, C.c_void_p), pl.n_ops, C.sizeof(S.PlanOp), pl.arena_bytes,
-                                                   C.byref(h)), 'ds_unet_create')
-                if self.cuda_graph:
-                    px = self.img_channels * self.img_resolution ** 2 * 4
-                    T, cd = pl.meta['ctx_tokens'], self.info['ctx_dim']
-                    io_bytes = (C.c_size_t * 6)(B * px, Bt * px, nT * 4, (B if nT > 1 else 1) * 16, Bt * 64 * 4, Bt * T * cd * 4)
-                    _lib.check(self.lib.ds_unet_enable_graph(h, io_bytes, 6), 'ds_unet_enable_graph')
-            ent = (h, pl)
-            self._plans[key] = ent
-        return ent
+        px = self.img_channels * self.img_resolution ** 2 * 4
+        return self.native.get((B, Bt, nT),
+                               lambda: ldm_plan.compile_ldm_plan(self.st, self.wb, self.info, B, Bt, nT, self.img_resolution, npass=self.npass,
+                                                                 flash_attn=self.flash_attn, f8=self.f8, f8_linear=self.f8_linear),
+                               (lambda pl: (B * px, Bt * px, nT * 4, (B if nT > 1 else 1) * 16, Bt * 64 * 4,
+                                            Bt * pl.meta['ctx_tokens'] * self.info['ctx_dim'] * 4)) if self.cuda_graph else None)
 
     def eps(self, x_scaled_src, coef, tvals, context, bottleneck=None):
         """eps-net on Bt = context.shape[0] samples: inputs x [B,...] (c_in applied in-kernel via coef[:,2]), timesteps tvals [1|Bt]."""
@@ -135,11 +112,9 @@ class B200LDMNet:
         nT = tvals.numel()
         h, pl = self._plan(B, Bt, nT)
         out = torch.empty((Bt,) + tuple(x_scaled_src.shape[1:]), device=x_scaled_src.device)
-        io = (C.c_void_p * 6)(x_scaled_src.data_ptr(), out.data_ptr(), tvals.data_ptr(), coef.data_ptr(),
-                              bottleneck.data_ptr() if bottleneck is not None else None, context.data_ptr())
-        stream = torch.cuda.current_stream(x_scaled_src.device).cuda_stream
-        _lib.check(self.lib.ds_unet_forward_io(h, io, 6, C.c_void_p(stream)), 'ds_unet_forward_io')
-        self.total_launches += self.lib.ds_unet_last_launch_count(h)
+        io = (x_scaled_src.data_ptr(), out.data_ptr(), tvals.data_ptr(), coef.data_ptr(), bottleneck.data_ptr() if bottleneck is not None else None,
+              context.data_ptr())
+        self.total_launches += self.native.run(h, io, torch.cuda.current_stream(x_scaled_src.device).cuda_stream)
         return out
 
     # ---- the reference-facing call (networks_edm.py:670-692) -------------------------------------------------------------------
@@ -192,11 +167,11 @@ class B200LDMNet:
     def profile_call(self, x, sigma, condition, unconditional_condition=None):
         """One denoiser call with per-op CUDA-event timing -> {op_type: (count, total_ms)} and per-op list [(type, tag, ms)]."""
         self(x, sigma, condition=condition, unconditional_condition=unconditional_condition)
-        for (h, pl) in self._plans.values():
+        for (h, pl) in self.native.plans.values():
             self.lib.ds_unet_set_profiling(h, 1)
         self(x, sigma, condition=condition, unconditional_condition=unconditional_condition)
         out, per_op = {}, []
-        for (h, pl) in self._plans.values():
+        for (h, pl) in self.native.plans.values():
             buf = (C.c_float * pl.n_ops)()
             n = self.lib.ds_unet_get_profile(h, buf, pl.n_ops)
             self.lib.ds_unet_set_profiling(h, 0)
@@ -208,14 +183,6 @@ class B200LDMNet:
                 out[t] = (c + 1, ms + buf[i])
                 per_op.append((t, pl.ops_array[i].tag, buf[i]))
         return out, per_op
-
-    def __del__(self):
-        try:
-            for h, _ in self._plans.values():
-                self.lib.ds_unet_destroy(h)
-            self.lib.ds_weights_destroy(self._wh)
-        except Exception:
-            pass
 
     def eval(self):
         return self

@@ -19,26 +19,13 @@ import torch
 
 from . import _cstructs as S
 from . import gemm_desc as G
-from .plan import Plan, WeightBlob, _Arena
+from .plan import F4, H2, NPL, PlanBuilder, WeightBlob, io
 
-F4, H2 = 4, 2
 CTX_TOKENS_PITCH = 128        # P / V^T row pitch for the 77 context tokens (multiple of 8 elements for TMA strides)
-
-
-def _groups(c):
-    """LDM uses GroupNorm32(32, channels) everywhere (util.py:202-216, attention.py:76-77): always 32 groups."""
-    assert c % 32 == 0
-    return 32
 
 
 def dpad(d):
     return -(-d // 64) * 64
-
-
-def prows(n):
-    """Row count of a weight packed by gemm_desc.pack_conv_weight (padded to whole N tiles)."""
-    bn, tiles = G.pick_bn(n)
-    return bn * tiles
 
 
 def ldm_structure(params, num_heads):
@@ -108,24 +95,10 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False):
     wb = WeightBlob()
     info = dict(res=[], ctx_dim=None, f8_shift={})
 
-    def add_lin(key, w, bias=None, as_f8=False):
-        """Linear / 1x1 conv weight [N, K] as a packed GEMM operand."""
-        if as_f8:
-            packed, info['f8_shift'][key] = G.pack_conv_weight_f8(w.reshape(w.shape[0], w.shape[1], 1, 1))
-            wb.add(key + ':w', packed)
-        else:
-            wb.add(key + ':w', G.pack_conv_weight(w.reshape(w.shape[0], w.shape[1], 1, 1)))
-        if bias is not None:
-            wb.add(key + ':b', bias)
-
     def add_conv(key, w, skip_w=None, bias=None, as_f8=False):
+        shift = wb.add_gemm(key, w, skip_w, bias, f8=as_f8)[1]
         if as_f8:
-            packed, info['f8_shift'][key] = G.pack_conv_weight_f8(w, skip_w)
-            wb.add(key + ':w', packed)
-        else:
-            wb.add(key + ':w', G.pack_conv_weight(w, skip_w))
-        if bias is not None:
-            wb.add(key + ':b', bias)
+            info['f8_shift'][key] = shift
 
     for k in ('time_embed.0', 'time_embed.2'):
         wb.add(k + ':w', P(k + '.weight'))
@@ -138,11 +111,9 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False):
             if kind == 'conv':
                 add_conv(n, P(n + '.weight'), bias=P(n + '.bias'))
             elif kind == 'res':
-                wb.add(n + '.n0:g', P(n + '.in_layers.0.weight'))
-                wb.add(n + '.n0:b', P(n + '.in_layers.0.bias'))
+                wb.add_norm(n + '.n0', P, n + '.in_layers.0')
                 add_conv(n + '.c0', P(n + '.in_layers.2.weight'), bias=P(n + '.in_layers.2.bias'), as_f8=f8)
-                wb.add(n + '.n1:g', P(n + '.out_layers.0.weight'))
-                wb.add(n + '.n1:b', P(n + '.out_layers.0.bias'))
+                wb.add_norm(n + '.n1', P, n + '.out_layers.0')
                 b1 = P(n + '.out_layers.3.bias')
                 skw = None
                 if (n + '.skip_connection.weight') in params:
@@ -156,26 +127,24 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False):
             elif kind == 'attn':
                 _, _, ch, heads, dh = L
                 t = n + '.transformer_blocks.0'
-                wb.add(n + '.norm:g', P(n + '.norm.weight'))
-                wb.add(n + '.norm:b', P(n + '.norm.bias'))
-                add_lin(n + '.proj_in', P(n + '.proj_in.weight').reshape(heads * dh, ch), P(n + '.proj_in.bias'), as_f8=f8_linear)
+                wb.add_norm(n + '.norm', P)
+                add_conv(n + '.proj_in', P(n + '.proj_in.weight').reshape(heads * dh, ch), bias=P(n + '.proj_in.bias'), as_f8=f8_linear)
                 for k in (1, 2, 3):
-                    wb.add(f'{t}.norm{k}:g', P(f'{t}.norm{k}.weight'))
-                    wb.add(f'{t}.norm{k}:b', P(f'{t}.norm{k}.bias'))
+                    wb.add_norm(f'{t}.norm{k}', P)
                 # self-attention: [q | k] rows for one GEMM, v as the M operand of the V^T GEMM
                 wq, wk, wv = (_pad_heads_rows(P(f'{t}.attn1.to_{x}.weight'), heads, dh) for x in 'qkv')
-                add_lin(t + '.attn1.qk', torch.cat([wq, wk]))
+                add_conv(t + '.attn1.qk', torch.cat([wq, wk]))
                 wb.add(t + '.attn1.v:w', G.split_planes(wv))
-                add_lin(t + '.attn1.out', _pad_heads_cols(P(t + '.attn1.to_out.0.weight'), heads, dh), P(t + '.attn1.to_out.0.bias'))
+                add_conv(t + '.attn1.out', _pad_heads_cols(P(t + '.attn1.to_out.0.weight'), heads, dh), bias=P(t + '.attn1.to_out.0.bias'))
                 # cross-attention
-                add_lin(t + '.attn2.q', _pad_heads_rows(P(t + '.attn2.to_q.weight'), heads, dh), as_f8=f8_linear)
-                add_lin(t + '.attn2.k', _pad_heads_rows(P(t + '.attn2.to_k.weight'), heads, dh))
+                add_conv(t + '.attn2.q', _pad_heads_rows(P(t + '.attn2.to_q.weight'), heads, dh), as_f8=f8_linear)
+                add_conv(t + '.attn2.k', _pad_heads_rows(P(t + '.attn2.to_k.weight'), heads, dh))
                 wb.add(t + '.attn2.v:w', G.split_planes(_pad_heads_rows(P(t + '.attn2.to_v.weight'), heads, dh)))
-                add_lin(t + '.attn2.out', _pad_heads_cols(P(t + '.attn2.to_out.0.weight'), heads, dh), P(t + '.attn2.to_out.0.bias'))
+                add_conv(t + '.attn2.out', _pad_heads_cols(P(t + '.attn2.to_out.0.weight'), heads, dh), bias=P(t + '.attn2.to_out.0.bias'))
                 info['ctx_dim'] = P(t + '.attn2.to_k.weight').shape[1]
-                add_lin(t + '.ff1', P(t + '.ff.net.0.proj.weight'), P(t + '.ff.net.0.proj.bias'), as_f8=f8_linear)
-                add_lin(t + '.ff2', P(t + '.ff.net.2.weight'), P(t + '.ff.net.2.bias'), as_f8=f8_linear)
-                add_lin(n + '.proj_out', P(n + '.proj_out.weight').reshape(ch, heads * dh), P(n + '.proj_out.bias'), as_f8=f8_linear)
+                add_conv(t + '.ff1', P(t + '.ff.net.0.proj.weight'), bias=P(t + '.ff.net.0.proj.bias'), as_f8=f8_linear)
+                add_conv(t + '.ff2', P(t + '.ff.net.2.weight'), bias=P(t + '.ff.net.2.bias'), as_f8=f8_linear)
+                add_conv(n + '.proj_out', P(n + '.proj_out.weight').reshape(ch, heads * dh), bias=P(n + '.proj_out.bias'), as_f8=f8_linear)
             elif kind == 'down':
                 add_conv(n, P(n + '.op.weight'), bias=P(n + '.op.bias'))
             elif kind == 'up':
@@ -183,8 +152,7 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False):
     wb.add('affine:w', torch.cat(aff_w, dim=0))
     wb.add('affine:b', torch.cat(aff_b, dim=0))
     info['aff_total'] = aff_off
-    wb.add('out.0:g', P('out.0.weight'))
-    wb.add('out.0:b', P('out.0.bias'))
+    wb.add_norm('out.0', P)
     add_conv('out.2', P('out.2.weight'), bias=P('out.2.bias'))
     return wb, info
 
@@ -201,32 +169,18 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
 
     def f8_args(key):
         return dict(f8=True, acc_scale=2.0 ** -info['f8_shift'][key]) if key in info['f8_shift'] else {}
-    A = _Arena()
-    ops = []
-    npl = 2
-    io = lambda slot: S.ref(S.SPACE_IO, slot)
-    W = wb.ref
+    pb = PlanBuilder(wb, Bt, npass)
+    emit, W = pb.emit, wb.ref
     mc, ted = st['model_channels'], st['ted']
     cd = info['ctx_dim']
     T = ctx_tokens
     TP = CTX_TOKENS_PITCH
-    tag = [0]
-    emit = lambda b: ops.append((tag[0], b))
-    n_gn = sum(2 if L[0] == 'res' else (1 if L[0] == 'attn' else 0) for _, ls in st['inp'] + st['mid'] + st['out'] for L in ls) + 1
-    A.need('stats', n_gn * Bt * 32 * 2 * 8)
-    stat_i = [0]
-
-    def stats_slot():
-        i = stat_i[0]
-        stat_i[0] += 1
-        return i * Bt * 32 * 2 * 8
-
-    emit(lambda R_: S.MemsetDesc(ptr=R_('stats'), bytes=n_gn * Bt * 32 * 2 * 8))
+    pb.stats(sum(2 if L[0] == 'res' else (1 if L[0] == 'attn' else 0) for _, ls in st['inp'] + st['mid'] + st['out'] for L in ls) + 1)
     # ---------------- timestep embedding (util.py:151-171, openaimodel.py:723-724) + all emb_layers in one launch -------------
-    A.need('emb0', nT * mc * F4)
-    A.need('e1', nT * ted * F4)
-    A.need('e2', nT * ted * F4)
-    A.need('aff', nT * info['aff_total'] * F4)
+    pb.need('emb0', nT * mc * F4)
+    pb.need('e1', nT * ted * F4)
+    pb.need('e2', nT * ted * F4)
+    pb.need('aff', nT * info['aff_total'] * F4)
     emit(lambda R_: S.PosembDesc(sigma=io(S.DS_IO_SIGMA), nsig=nT, num_channels=mc, endpoint=0, swap_sincos=0, sigma_data=0.5, mode=1,
                                  coef=0, emb=R_('emb0')))
     emit(lambda R_: S.LinearDesc(in_=R_('emb0'), in_stride=mc if nT > 1 else 0, W=W('time_embed.0:w'), b=W('time_embed.0:b'), out=R_('e1'),
@@ -239,56 +193,31 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
     aff_stride = info['aff_total'] if nT > 1 else 0
     aff_off = dict(info['res'])
     # ---------------- context tokens -> fp16 planes (once per forward, shared by every cross-attention) ------------------------
-    A.need('ctx', npl * Bt * T * cd * H2)
-    emit(lambda R_: S.GnApplyDesc(src0=io(S.DS_IO_CTX), src1=0, C0=cd, C1=0, H=T, W=1, B=Bt, groups=32, sums=0, gamma=0, beta=0, eps=0.0,
-                                  silu=0, ada=0, ada_stride=0, resample=0, nplanes=npl, out_act=0, out_raw=R_('ctx'), out_raw_f32=0))
-
-    def gn_stats(slot, parts, hw):
-        (n0, c0), (n1, c1) = parts[0], (parts[1] if len(parts) > 1 else (None, 0))
-        emit(lambda R_: S.GnStatsDesc(src0=R_(n0), src1=R_(n1) if n1 else 0, C0=c0, C1=c1, HW=hw, B=Bt, groups=_groups(c0 + c1),
-                                      sums=R_('stats', slot)))
-
-    def gn_apply(slot, parts, H, g, b, eps, silu, out, fmt=0):
-        (n0, c0), (n1, c1) = parts[0], (parts[1] if len(parts) > 1 else (None, 0))
-        emit(lambda R_: S.GnApplyDesc(src0=R_(n0), src1=R_(n1) if n1 else 0, C0=c0, C1=c1, H=H, W=H, B=Bt, groups=_groups(c0 + c1),
-                                      sums=R_('stats', slot), gamma=W(g), beta=W(b), eps=eps, silu=silu, ada=0, ada_stride=0, resample=0,
-                                      nplanes=npl, out_act=R_(out), out_raw=0, out_raw_f32=0, fmt=fmt))
+    pb.need('ctx', NPL * Bt * T * cd * H2)
+    pb.to_planes(io(S.DS_IO_CTX), cd, T, 1, Bt, 'ctx')
 
     def lower_res(L, parts, H):
         """ResBlock (openaimodel.py:255-275): GN+SiLU+conv3x3, + Linear(SiLU(emb)), GN+SiLU+conv3x3, + skip (identity | 1x1)."""
         _, n, cin, cout = L
         M = Bt * H * H
         assert sum(c for _, c in parts) == cin
-        s0 = stats_slot()
-        gn_stats(s0, parts, H * H)
-        A.need('act', npl * M * max(cin, cout) * H2)
+        pb.need('act', NPL * M * max(cin, cout) * H2)
         has_skip = (n + '.c1:w') in wb.off and cin != cout
         if has_skip:
-            A.need('raw', npl * M * cin * H2)
-        (n0, c0), (n1, c1) = parts[0], (parts[1] if len(parts) > 1 else (None, 0))
-        emit(lambda R_: S.GnApplyDesc(src0=R_(n0), src1=R_(n1) if n1 else 0, C0=c0, C1=c1, H=H, W=H, B=Bt, groups=_groups(cin),
-                                      sums=R_('stats', s0), gamma=W(n + '.n0:g'), beta=W(n + '.n0:b'), eps=1e-5, silu=1, ada=0, ada_stride=0,
-                                      resample=0, nplanes=npl, out_act=R_('act'), out_raw=R_('raw') if has_skip else 0, out_raw_f32=0,
-                                      fmt=fmt_res))
-        A.need('y', M * cout * F4)
+            pb.need('raw', NPL * M * cin * H2)
+        pb.group_norm(parts, H, n + '.n0', 1e-5, 'act', raw='raw' if has_skip else None, fmt=fmt_res)
+        pb.need('y', M * cout * F4)
         off = aff_off[n]
         emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, cin, W(n + '.c0:w'), cout, taps=9, npass=npass, out_f32=R_('y'), bias=W(n + '.c0:b'),
                                     rowvec=R_('aff', off * F4), rowvec_stride=aff_stride, **f8_args(n + '.c0'))[0])
-        s1 = stats_slot()
-        gn_stats(s1, [('y', cout)], H * H)
-        gn_apply(s1, [('y', cout)], H, n + '.n1:g', n + '.n1:b', 1e-5, 1, 'act', fmt=fmt_res)
-        out = A.need('h:' + n, M * cout * F4)
+        pb.group_norm([('y', cout)], H, n + '.n1', 1e-5, 'act', fmt=fmt_res)
+        out = pb.need('h:' + n, M * cout * F4)
         res_name = None if has_skip else parts[0][0]
         assert has_skip or len(parts) == 1
         emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, cout, W(n + '.c1:w'), cout, taps=9, npass=npass, a2_ptr=R_('raw') if has_skip else 0,
                                     C2=cin if has_skip else 0, out_f32=R_(out), bias=W(n + '.c1:b'), residual=R_(res_name) if res_name else 0,
                                     ldr=cout, scale=1.0, **f8_args(n + '.c1'))[0])
         return out, cout
-
-    def cast_planes(src, C, H, dst, fmt=0):
-        """fp32 NHWC -> fp16 hi/lo planes, or the f8 operand image (fmt=1); no normalisation."""
-        emit(lambda R_: S.GnApplyDesc(src0=R_(src), src1=0, C0=C, C1=0, H=H, W=H, B=Bt, groups=32, sums=0, gamma=0, beta=0, eps=0.0, silu=0,
-                                      ada=0, ada_stride=0, resample=0, nplanes=npl, out_act=0, out_raw=R_(dst), out_raw_f32=0, fmt=fmt))
 
     def lower_attn(L, src, H):
         """SpatialTransformer with one BasicTransformerBlock (attention.py:250-261, :211-215)."""
@@ -298,91 +227,63 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
         hp = heads * dp
         Lq = H * H
         M = Bt * Lq
-        s0 = stats_slot()
-        gn_stats(s0, [(src, ch)], Lq)
-        A.need('act', npl * M * max(ch, inner) * H2)
-        gn_apply(s0, [(src, ch)], H, n + '.norm:g', n + '.norm:b', 1e-6, 0, 'act', fmt=fmt_lin)
+        pb.need('act', NPL * M * max(ch, inner) * H2)
+        pb.group_norm([(src, ch)], H, n + '.norm', 1e-6, 'act', silu=0, fmt=fmt_lin)
         for nm in ('t0', 't1', 't2', 't3'):
-            A.need(nm, M * inner * F4)
+            pb.need(nm, M * inner * F4)
         emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, ch, W(n + '.proj_in:w'), inner, taps=1, npass=npass, out_f32=R_('t0'),
-                                    bias=W(n + '.proj_in:b'), **(f8_args(n + '.proj_in') if f8_linear else {}))[0])
-        A.need('ln', npl * M * inner * H2)
-        A.need('qk', npl * M * 2 * hp * H2)
-        A.need('vt', npl * Bt * hp * max(Lq, TP) * H2)
-        if not (flash_attn and dp == 64 and npl == 2):
-            A.need('S', Bt * heads * Lq * max(Lq, 80) * F4)
-            A.need('P', npl * Bt * heads * Lq * max(Lq, TP) * H2)
-        A.need('o', npl * M * hp * H2)
+                                    bias=W(n + '.proj_in:b'), **f8_args(n + '.proj_in'))[0])
+        pb.need('ln', NPL * M * inner * H2)
+        pb.need('qk', NPL * M * 2 * hp * H2)
+        pb.need('vt', NPL * Bt * hp * max(Lq, TP) * H2)
+        # fused QK^T -> softmax -> PV (attention.cu): at 64x64 latents the 4096 x 4096 score matrix per head never reaches HBM
+        fused = flash_attn and dp == 64
 
         def ln(k, srcbuf, fmt=0):
             emit(lambda R_: S.LayernormDesc(src=R_(srcbuf), gamma=W(f'{t}.norm{k}:g'), beta=W(f'{t}.norm{k}:b'), out=R_('ln'), rows=M, C=inner,
-                                            nplanes=npl, eps=1e-5, fmt=fmt))
+                                            nplanes=NPL, eps=1e-5, fmt=fmt))
         # ---- self-attention (attn1): x = attn1(norm1(x)) + x
         ln(1, 't0')
         emit(lambda R_: G.conv_gemm(R_('ln'), Bt, H, H, inner, W(t + '.attn1.qk:w'), 2 * hp, taps=1, npass=npass, out_h16=R_('qk'))[0])
-        emit(lambda R_: G.rows_gemm(W(t + '.attn1.v:w'), hp, inner, 1, R_('ln'), Lq, inner, Bt, inner, num_z=Bt, nh=1, m_valid=hp, n_valid=Lq,
-                                    npass=npass, b_z_per_zb=1, out_h16=R_('vt'), o_zb=hp * Lq, ldo=Lq, o_plane=Bt * hp * Lq)[0])
-        flash = flash_attn and dp == 64 and npl == 2
-        if flash:
-            # fused QK^T -> softmax -> PV (attention.cu): at 64x64 latents the 4096 x 4096 score matrix per head never reaches HBM
-            emit(lambda R_: S.AttnDesc(q=R_('qk'), k=R_('qk'), vt=R_('vt'), out=R_('o'), B=Bt, nh=heads, L=Lq, Lk=Lq, q_pitch=2 * hp, q_c0=0,
-                                       k_pitch=2 * hp, k_c0=hp, vt_pitch=Lq, o_pitch=hp, nplanes=npl, scale=dh ** -0.5))
-        else:
-            emit(lambda R_: G.rows_gemm(R_('qk'), Lq, 2 * hp, Bt, R_('qk'), Lq, 2 * hp, Bt, dp, num_z=Bt * heads, nh=heads, m_valid=Lq, n_valid=Lq,
-                                        npass=npass, a_c_per_zh=dp, a_n_per_zb=1, b_k0=hp, b_k_per_zh=dp, b_z_per_zb=1, out_f32=R_('S'),
-                                        o_zb=heads * Lq * Lq, o_zh=Lq * Lq, ldo=Lq, scale=dh ** -0.5)[0])
-            emit(lambda R_: S.SoftmaxDesc(S=R_('S'), P=R_('P'), rows=Bt * heads * Lq, L=Lq, nplanes=npl, pitch_in=0, pitch_out=0))
-            emit(lambda R_: G.rows_gemm(R_('P'), Lq, Lq, Bt * heads, R_('vt'), hp, Lq, Bt, Lq, num_z=Bt * heads, nh=heads, m_valid=Lq, n_valid=dp,
-                                        npass=npass, a_n_per_zb=heads, a_n_per_zh=1, b_row_per_zh=dp, b_z_per_zb=1, out_h16=R_('o'),
-                                        o_zb=Lq * hp, o_zh=dp, ldo=hp, o_plane=M * hp)[0])
+        pb.vt_gemm(t + '.attn1.v:w', 'ln', inner, hp, Lq, Lq)
+        pb.attention(fused, 'qk', 'qk', 'o', heads, Lq, Lq, dp, dh ** -0.5, Lq)
+        pb.need('o', NPL * M * hp * H2)
         emit(lambda R_: G.conv_gemm(R_('o'), Bt, H, H, hp, W(t + '.attn1.out:w'), inner, taps=1, npass=npass, out_f32=R_('t1'),
                                     bias=W(t + '.attn1.out:b'), residual=R_('t0'), ldr=inner)[0])
         # ---- cross-attention (attn2): x = attn2(norm2(x), context) + x
         ln(2, 't1', fmt=fmt_lin)           # single consumer: the to_q GEMM below
-        A.need('q2', npl * M * hp * H2)
-        A.need('k2', npl * Bt * T * hp * H2)
+        pb.need('q2', NPL * M * hp * H2)
+        pb.need('k2', NPL * Bt * T * hp * H2)
         emit(lambda R_: G.conv_gemm(R_('ln'), Bt, H, H, inner, W(t + '.attn2.q:w'), hp, taps=1, npass=npass, out_h16=R_('q2'),
-                                    **(f8_args(t + '.attn2.q') if f8_linear else {}))[0])
-        emit(lambda R_: G.rows_gemm(R_('ctx'), Bt * T, cd, 1, W(t + '.attn2.k:w'), prows(hp), cd, 1, cd, num_z=1, nh=1, m_valid=Bt * T, n_valid=hp,
-                                    npass=npass, out_h16=R_('k2'), ldo=hp, o_plane=Bt * T * hp)[0])
-        emit(lambda R_: G.rows_gemm(W(t + '.attn2.v:w'), hp, cd, 1, R_('ctx'), T, cd, Bt, cd, num_z=Bt, nh=1, m_valid=hp, n_valid=T,
-                                    npass=npass, b_z_per_zb=1, out_h16=R_('vt'), o_zb=hp * TP, ldo=TP, o_plane=Bt * hp * TP)[0])
-        if flash:
-            emit(lambda R_: S.AttnDesc(q=R_('q2'), k=R_('k2'), vt=R_('vt'), out=R_('o'), B=Bt, nh=heads, L=Lq, Lk=T, q_pitch=hp, q_c0=0,
-                                       k_pitch=hp, k_c0=0, vt_pitch=TP, o_pitch=hp, nplanes=npl, scale=dh ** -0.5))
-        else:
-            emit(lambda R_: G.rows_gemm(R_('q2'), Lq, hp, Bt, R_('k2'), T, hp, Bt, dp, num_z=Bt * heads, nh=heads, m_valid=Lq, n_valid=T,
-                                        npass=npass, a_c_per_zh=dp, a_n_per_zb=1, b_k_per_zh=dp, b_z_per_zb=1, out_f32=R_('S'),
-                                        o_zb=heads * Lq * 80, o_zh=Lq * 80, ldo=80, scale=dh ** -0.5)[0])
-            emit(lambda R_: S.SoftmaxDesc(S=R_('S'), P=R_('P'), rows=Bt * heads * Lq, L=T, nplanes=npl, pitch_in=80, pitch_out=TP))
-            emit(lambda R_: G.rows_gemm(R_('P'), Lq, TP, Bt * heads, R_('vt'), hp, TP, Bt, TP, num_z=Bt * heads, nh=heads, m_valid=Lq, n_valid=dp,
-                                        npass=npass, a_n_per_zb=heads, a_n_per_zh=1, b_row_per_zh=dp, b_z_per_zb=1, out_h16=R_('o'),
-                                        o_zb=Lq * hp, o_zh=dp, ldo=hp, o_plane=M * hp, a_k_valid=T, b_k_valid=T)[0])
+                                    **f8_args(t + '.attn2.q'))[0])
+        emit(lambda R_: G.rows_gemm(R_('ctx'), Bt * T, cd, 1, W(t + '.attn2.k:w'), G.padded_rows(hp), cd, 1, cd, num_z=1, nh=1, m_valid=Bt * T,
+                                    n_valid=hp, npass=npass, out_h16=R_('k2'), ldo=hp, o_plane=Bt * T * hp)[0])
+        pb.vt_gemm(t + '.attn2.v:w', 'ctx', cd, hp, T, TP)
+        pb.attention(fused, 'q2', 'k2', 'o', heads, Lq, T, dp, dh ** -0.5, TP, s_pitch=80)
         emit(lambda R_: G.conv_gemm(R_('o'), Bt, H, H, hp, W(t + '.attn2.out:w'), inner, taps=1, npass=npass, out_f32=R_('t2'),
                                     bias=W(t + '.attn2.out:b'), residual=R_('t1'), ldr=inner)[0])
         # ---- GEGLU feed-forward: x = ff(norm3(x)) + x
         ln(3, 't2', fmt=fmt_lin)
-        A.need('ff', M * 8 * inner * F4)
-        A.need('gg', npl * M * 4 * inner * H2)
+        pb.need('ff', M * 8 * inner * F4)
+        pb.need('gg', NPL * M * 4 * inner * H2)
         emit(lambda R_: G.conv_gemm(R_('ln'), Bt, H, H, inner, W(t + '.ff1:w'), 8 * inner, taps=1, npass=npass, out_f32=R_('ff'),
-                                    bias=W(t + '.ff1:b'), **(f8_args(t + '.ff1') if f8_linear else {}))[0])
-        emit(lambda R_: S.GegluDesc(src=R_('ff'), out=R_('gg'), rows=M, I=4 * inner, nplanes=npl, fmt=fmt_lin))
+                                    bias=W(t + '.ff1:b'), **f8_args(t + '.ff1'))[0])
+        emit(lambda R_: S.GegluDesc(src=R_('ff'), out=R_('gg'), rows=M, I=4 * inner, nplanes=NPL, fmt=fmt_lin))
         emit(lambda R_: G.conv_gemm(R_('gg'), Bt, H, H, 4 * inner, W(t + '.ff2:w'), inner, taps=1, npass=npass, out_f32=R_('t3'),
-                                    bias=W(t + '.ff2:b'), residual=R_('t2'), ldr=inner, **(f8_args(t + '.ff2') if f8_linear else {}))[0])
+                                    bias=W(t + '.ff2:b'), residual=R_('t2'), ldr=inner, **f8_args(t + '.ff2'))[0])
         # ---- proj_out + outer residual
-        cast_planes('t3', inner, H, 'ln', fmt=fmt_lin)
-        out = A.need('h:' + n, M * ch * F4)
+        pb.to_planes('t3', inner, H, H, Bt, 'ln', fmt=fmt_lin)
+        out = pb.need('h:' + n, M * ch * F4)
         emit(lambda R_: G.conv_gemm(R_('ln'), Bt, H, H, inner, W(n + '.proj_out:w'), ch, taps=1, npass=npass, out_f32=R_(out),
-                                    bias=W(n + '.proj_out:b'), residual=R_(src), ldr=ch, **(f8_args(n + '.proj_out') if f8_linear else {}))[0])
+                                    bias=W(n + '.proj_out:b'), residual=R_(src), ldr=ch, **f8_args(n + '.proj_out'))[0])
         return out, ch
 
     def lower_down(L, src, H):
         _, n, cin, cout = L
         Ho = H // 2
-        A.need('s2d', npl * Bt * H * H * cin * H2)
-        emit(lambda R_: S.GnApplyDesc(src0=R_(src), src1=0, C0=cin, C1=0, H=H, W=H, B=Bt, groups=32, sums=0, gamma=0, beta=0, eps=0.0, silu=0,
-                                      ada=0, ada_stride=0, resample=3, nplanes=npl, out_act=0, out_raw=R_('s2d'), out_raw_f32=0))
-        out = A.need('h:' + n, Bt * Ho * Ho * cout * F4)
+        pb.need('s2d', NPL * Bt * H * H * cin * H2)
+        pb.to_planes(src, cin, H, H, Bt, 's2d', resample=3)
+        out = pb.need('h:' + n, Bt * Ho * Ho * cout * F4)
         emit(lambda R_: G.conv_gemm(R_('s2d'), Bt, Ho, Ho, cin, W(n + ':w'), cout, taps=9, npass=npass, out_f32=R_(out), bias=W(n + ':b'),
                                     s2d=True)[0])
         return out, cout, Ho
@@ -390,28 +291,27 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
     def lower_up(L, src, H):
         _, n, cin, cout = L
         Ho = H * 2
-        A.need('act', npl * Bt * Ho * Ho * cin * H2)
-        emit(lambda R_: S.GnApplyDesc(src0=R_(src), src1=0, C0=cin, C1=0, H=H, W=H, B=Bt, groups=32, sums=0, gamma=0, beta=0, eps=0.0, silu=0,
-                                      ada=0, ada_stride=0, resample=2, nplanes=npl, out_act=0, out_raw=R_('act'), out_raw_f32=0, fmt=fmt_res))
-        out = A.need('h:' + n, Bt * Ho * Ho * cout * F4)
+        pb.need('act', NPL * Bt * Ho * Ho * cin * H2)
+        pb.to_planes(src, cin, H, H, Bt, 'act', fmt=fmt_res, resample=2)
+        out = pb.need('h:' + n, Bt * Ho * Ho * cout * F4)
         emit(lambda R_: G.conv_gemm(R_('act'), Bt, Ho, Ho, cin, W(n + ':w'), cout, taps=9, npass=npass, out_f32=R_(out), bias=W(n + ':b'),
                                     **f8_args(n))[0])
         return out, cout, Ho
 
     # ---------------- input conv --------------------------------------------------------------------------------------------
     cimg = st['in_channels']
-    A.need('in_planes', npl * Bt * R * R * 64 * H2)
+    pb.need('in_planes', NPL * Bt * R * R * 64 * H2)
     emit(lambda R_: S.PrepInputDesc(x=io(S.DS_IO_X), coef=io(S.DS_IO_LABELS), coef_stride=4 if B > 1 and nT > 1 else 0, B=Bt, C=cimg,
-                                    HW=R * R, nplanes=npl, x_batch=B, out=R_('in_planes')))
+                                    HW=R * R, nplanes=NPL, x_batch=B, out=R_('in_planes')))
     first = st['inp'][0][1][0]
-    h = A.need('h:' + first[1], Bt * R * R * first[3] * F4)
+    h = pb.need('h:' + first[1], Bt * R * R * first[3] * F4)
     emit(lambda R_: G.conv_gemm(R_('in_planes'), Bt, R, R, 64, W(first[1] + ':w'), first[3], taps=9, npass=npass, out_f32=R_(h),
                                 bias=W(first[1] + ':b'))[0])
     cur, cur_c, H = h, first[3], R
     hs = [(cur, cur_c)]
     for _, layers in st['inp'][1:]:
         for L in layers:
-            tag[0] += 1
+            pb.tag += 1
             if L[0] == 'res':
                 cur, cur_c = lower_res(L, [(cur, cur_c)], H)
             elif L[0] == 'attn':
@@ -420,7 +320,7 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
                 cur, cur_c, H = lower_down(L, cur, H)
         hs.append((cur, cur_c))
     for L in st['mid'][0][1]:
-        tag[0] += 1
+        pb.tag += 1
         if L[0] == 'res':
             cur, cur_c = lower_res(L, [(cur, cur_c)], H)
         else:
@@ -431,7 +331,7 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
         sk, sc = hs.pop()
         first_layer = True
         for L in layers:
-            tag[0] += 1
+            pb.tag += 1
             if L[0] == 'res':
                 parts = [(cur, cur_c), (sk, sc)] if first_layer else [(cur, cur_c)]
                 cur, cur_c = lower_res(L, parts, H)
@@ -441,24 +341,11 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
                 cur, cur_c, H = lower_up(L, cur, H)
             first_layer = False
     # ---------------- out: GN + SiLU + conv3x3 -> eps (NCHW) -----------------------------------------------------------------
-    tag[0] += 1
-    so = stats_slot()
-    gn_stats(so, [(cur, cur_c)], H * H)
-    A.need('act', npl * Bt * H * H * cur_c * H2)
-    gn_apply(so, [(cur, cur_c)], H, 'out.0:g', 'out.0:b', 1e-5, 1, 'act')
+    pb.tag += 1
+    pb.need('act', NPL * Bt * H * H * cur_c * H2)
+    pb.group_norm([(cur, cur_c)], H, 'out.0', 1e-5, 'act')
     fin_c = cur_c
     emit(lambda R_: G.conv_gemm(R_('act'), Bt, R, R, fin_c, W('out.2:w'), st['out_channels'], taps=9, npass=npass, bias=W('out.2:b'),
-                                edm=(0, 0, 0, st['out_channels'], io(S.DS_IO_D)))[0])
-    assert stat_i[0] <= n_gn and H == R
-
-    total = A.finalize()
-    arr = (S.PlanOp * len(ops))()
-    for i, (tg, builder) in enumerate(ops):
-        desc = builder(A.ref)
-        if isinstance(desc, S.GemmDesc) and desc.edm_out == 1 and desc.edm_x == 0:
-            desc.edm_out = 2                       # plain NCHW write of eps
-        arr[i].type = S.OP_TYPE_OF[type(desc)]
-        arr[i].tag = tg
-        setattr(arr[i].u, S.UNION_FIELD[arr[i].type], desc)
-    meta = dict(B=B, Bt=Bt, nT=nT, npass=npass, ctx_tokens=ctx_tokens, n_ops=len(ops), n_gemm=sum(1 for i in range(len(ops)) if arr[i].type == S.DS_OP_GEMM))
-    return Plan(arr, len(ops), total, dict(A.offsets), meta)
+                                nchw_out=(st['out_channels'], io(S.DS_IO_D)))[0])
+    assert H == R
+    return pb.finish(B=B, Bt=Bt, nT=nT, npass=npass, ctx_tokens=ctx_tokens)

@@ -9,7 +9,6 @@ from collections import OrderedDict
 
 import torch
 
-from . import _cstructs as S
 from . import _lib
 from . import edm_nets
 from . import plan as planner
@@ -58,11 +57,8 @@ class B200Net:
         self.spec.sigma_data = sigma_data
         self.wb, self.winfo = planner.pack_weights(self.spec, params, f8=self.f8, f8_min_channels=self.f8_min_channels)
         blob = self.wb.bytes()
-        self._wh = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.ds_weights_create(blob, len(blob), C.byref(self._wh)), 'ds_weights_create')
+        self.native = _lib.NativePlans(blob, self.device)
         self.weight_bytes = len(blob)
-        self._plans = {}
         self.launches_last_forward = 0
         self.total_launches = 0
 
@@ -96,24 +92,16 @@ class B200Net:
         return net
 
     # ---- plan cache -------------------------------------------------------------------------------------------------
+    @property
+    def _plans(self):
+        return self.native.plans
+
     def _plan(self, B, nsig, nlab):
-        key = (B, nsig, nlab)
-        ent = self._plans.get(key)
-        if ent is None:
-            import os
-            pl = planner.compile_plan(self.spec, self.wb, self.winfo, B, nsig, nlab, npass=self.npass, fuse_stats=self.fuse_stats,
-                                           flash_attn=self.flash_attn, f8=self.f8, gn_coef=os.environ.get('DSB_GN_COEF', '1') != '0')
-            h = C.c_void_p()
-            with torch.cuda.device(self.device):
-                _lib.check(self.lib.ds_unet_create(self._wh, C.cast(pl.ops_array, C.c_void_p), pl.n_ops, C.sizeof(S.PlanOp),
-                                                   pl.arena_bytes, C.byref(h)), 'ds_unet_create')
-                if self.cuda_graph:
-                    img = B * self.img_channels * self.img_resolution ** 2 * 4
-                    io_bytes = (C.c_size_t * 6)(img, img, nsig * 4, nlab * self.label_dim * 4, B * 64 * 4, 0)
-                    _lib.check(self.lib.ds_unet_enable_graph(h, io_bytes, 6), 'ds_unet_enable_graph')
-            ent = (h, pl)
-            self._plans[key] = ent
-        return ent
+        img = B * self.img_channels * self.img_resolution ** 2 * 4
+        return self.native.get((B, nsig, nlab),
+                               lambda: planner.compile_plan(self.spec, self.wb, self.winfo, B, nsig, nlab, npass=self.npass,
+                                                            fuse_stats=self.fuse_stats, flash_attn=self.flash_attn, f8=self.f8),
+                               (lambda pl: (img, img, nsig * 4, nlab * self.label_dim * 4, B * 64 * 4, 0)) if self.cuda_graph else None)
 
     # ---- the reference-facing call ----------------------------------------------------------------------------------
     def __call__(self, x, sigma, class_labels=None, out=None, bottleneck=None, **_):
@@ -141,10 +129,8 @@ class B200Net:
         if out is None:
             out = torch.empty_like(x)
         stream = torch.cuda.current_stream(x.device).cuda_stream
-        rc = self.lib.ds_unet_forward(h, x.data_ptr(), sig.data_ptr(), lab.data_ptr() if lab is not None else None, out.data_ptr(),
-                                      bottleneck.data_ptr() if bottleneck is not None else None, C.c_void_p(stream))
-        _lib.check(rc, 'ds_unet_forward')
-        self.launches_last_forward = self.lib.ds_unet_last_launch_count(h)
+        self.launches_last_forward = self.native.run(h, (x.data_ptr(), out.data_ptr(), sig.data_ptr(), lab.data_ptr() if lab is not None else None,
+                                                         bottleneck.data_ptr() if bottleneck is not None else None, None), stream)
         self.total_launches += self.launches_last_forward
         return out
 
@@ -174,20 +160,8 @@ class B200Net:
 
     def debug_read(self, B, nsig, nlab, name, numel, dtype=torch.float32):
         """Copy a named workspace buffer of the plan for (B, nsig, nlab) to the host (tests only)."""
-        h, pl = self._plan(B, nsig, nlab)
-        t = torch.empty(numel, dtype=dtype)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(self.lib.ds_unet_debug_read(h, pl.arena_offsets[name], t.data_ptr(), t.numel() * t.element_size(), C.c_void_p(stream)),
-                   'ds_unet_debug_read')
-        return t
-
-    def __del__(self):
-        try:
-            for h, _ in self._plans.values():
-                self.lib.ds_unet_destroy(h)
-            self.lib.ds_weights_destroy(self._wh)
-        except Exception:
-            pass
+        self._plan(B, nsig, nlab)
+        return self.native.debug_read((B, nsig, nlab), name, numel, dtype)
 
     # torch.nn.Module-ish conveniences used by sample.py-style callers
     def eval(self):

@@ -4,16 +4,13 @@ images = Decoder(post_quant_conv(z / scale_factor)).  OPT-IN, not yet run on har
     vae = B200VAEDecoder.from_reference(net.model)            # net.model: the LatentDiffusion object behind CFGPrecond
     images = vae.decode(latents)                              # instead of net.model.decode_first_stage(latents)
 """
-import ctypes as C
 from collections import OrderedDict
 
 import torch
 
-from . import _cstructs as S
 from . import _lib
 from . import vae_plan
-
-PRECISIONS = {'fp16x3': 3, 'fp16': 1}
+from .net import PRECISIONS
 
 
 class B200VAEDecoder:
@@ -23,14 +20,12 @@ class B200VAEDecoder:
             raise _lib.DsError('B200VAEDecoder needs a CUDA device (no CPU fallback)')
         self.lib = _lib.load()
         self.scale_factor = float(scale_factor)
+        if precision not in ('fp16x3', 'fp16'):
+            raise ValueError(f'precision {precision!r}: the VAE decoder runs fp16x3 or fp16')
         self.npass = PRECISIONS[precision]
         self.mods, self.meta = vae_plan.vae_structure(params)
         self.wb = vae_plan.pack_vae_weights(self.mods, self.meta, params)
-        blob = self.wb.bytes()
-        self._wh = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.ds_weights_create(blob, len(blob), C.byref(self._wh)), 'ds_weights_create')
-        self._plans = {}
+        self.native = _lib.NativePlans(self.wb.bytes(), self.device)
         self._coef = torch.tensor([[0.0, 0.0, 1.0 / self.scale_factor, 0.0]], device=self.device)
         self.total_launches = 0
 
@@ -42,16 +37,7 @@ class B200VAEDecoder:
         return cls(sd, scale_factor=float(ldm_model.scale_factor), **kw)
 
     def _plan(self, B, R):
-        ent = self._plans.get((B, R))
-        if ent is None:
-            pl = vae_plan.compile_vae_plan(self.mods, self.meta, self.wb, B, R, npass=self.npass)
-            h = C.c_void_p()
-            with torch.cuda.device(self.device):
-                _lib.check(self.lib.ds_unet_create(self._wh, C.cast(pl.ops_array, C.c_void_p), pl.n_ops, C.sizeof(S.PlanOp), pl.arena_bytes,
-                                                   C.byref(h)), 'ds_unet_create')
-            ent = (h, pl)
-            self._plans[(B, R)] = ent
-        return ent
+        return self.native.get((B, R), lambda: vae_plan.compile_vae_plan(self.mods, self.meta, self.wb, B, R, npass=self.npass))
 
     def decode(self, z, out=None):
         """z: [B, z_channels, R, R] latents as the samplers return them -> images [B, out_ch, s R, s R] (fp32, NCHW)."""
@@ -65,26 +51,12 @@ class B200VAEDecoder:
         s = self.meta['upscale']
         if out is None:
             out = torch.empty(B, self.meta['out_ch'], R * s, R * s, device=z.device)
-        io = (C.c_void_p * 6)(z.data_ptr(), out.data_ptr(), None, self._coef.data_ptr(), None, None)
-        stream = torch.cuda.current_stream(z.device).cuda_stream
-        _lib.check(self.lib.ds_unet_forward_io(h, io, 6, C.c_void_p(stream)), 'ds_unet_forward_io')
-        self.total_launches += self.lib.ds_unet_last_launch_count(h)
+        io = (z.data_ptr(), out.data_ptr(), None, self._coef.data_ptr(), None, None)
+        self.total_launches += self.native.run(h, io, torch.cuda.current_stream(z.device).cuda_stream)
         return out
 
     decode_first_stage = decode          # the reference's method name (ddpm.py:707)
 
     def debug_read(self, B, R, name, numel, dtype=torch.float32):
-        h, pl = self._plan(B, R)
-        t = torch.empty(numel, dtype=dtype)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        _lib.check(self.lib.ds_unet_debug_read(h, pl.arena_offsets[name], t.data_ptr(), t.numel() * t.element_size(), C.c_void_p(stream)),
-                   'ds_unet_debug_read')
-        return t
-
-    def __del__(self):
-        try:
-            for h, _ in self._plans.values():
-                self.lib.ds_unet_destroy(h)
-            self.lib.ds_weights_destroy(self._wh)
-        except Exception:
-            pass
+        self._plan(B, R)
+        return self.native.debug_read((B, R), name, numel, dtype)

@@ -17,9 +17,7 @@ import torch
 
 from . import _cstructs as S
 from . import gemm_desc as G
-from .plan import Plan, WeightBlob, _Arena
-
-F4, H2 = 4, 2
+from .plan import F4, H2, NPL, PlanBuilder, WeightBlob, io
 
 
 def vae_structure(params):
@@ -59,85 +57,58 @@ def pack_vae_weights(mods, meta, params):
     P = lambda k: params[k].detach().float().cpu()
     wb = WeightBlob()
 
-    def add_conv(key, w, skip_w=None, bias=None):
-        wb.add(key + ':w', G.pack_conv_weight(w, skip_w))
-        if bias is not None:
-            wb.add(key + ':b', bias)
-
-    def add_norm(key, n):
-        wb.add(key + ':g', P(n + '.weight'))
-        wb.add(key + ':b', P(n + '.bias'))
-
-    add_conv('post_quant_conv', P('post_quant_conv.weight'), bias=P('post_quant_conv.bias'))
+    wb.add_gemm('post_quant_conv', P('post_quant_conv.weight'), bias=P('post_quant_conv.bias'))
     for m in mods:
         n = m[1]
         if m[0] == 'conv':
-            add_conv(n, P(n + '.weight'), bias=P(n + '.bias'))
+            wb.add_gemm(n, P(n + '.weight'), bias=P(n + '.bias'))
         elif m[0] == 'res':
-            add_norm(n + '.n1', n + '.norm1')
-            add_conv(n + '.c1', P(n + '.conv1.weight'), bias=P(n + '.conv1.bias'))
-            add_norm(n + '.n2', n + '.norm2')
+            wb.add_norm(n + '.n1', P, n + '.norm1')
+            wb.add_gemm(n + '.c1', P(n + '.conv1.weight'), bias=P(n + '.conv1.bias'))
+            wb.add_norm(n + '.n2', P, n + '.norm2')
             b2, skw = P(n + '.conv2.bias'), None
             if (n + '.nin_shortcut.weight') in params:
                 skw = P(n + '.nin_shortcut.weight')
                 b2 = b2 + P(n + '.nin_shortcut.bias')
             assert (n + '.conv_shortcut.weight') not in params, '3x3 conv_shortcut is not lowered (SD-v1 uses nin_shortcut)'
-            add_conv(n + '.c2', P(n + '.conv2.weight'), skw, bias=b2)
+            wb.add_gemm(n + '.c2', P(n + '.conv2.weight'), skw, bias=b2)
         elif m[0] == 'attn':
             c = m[2]
-            add_norm(n + '.norm', n + '.norm')
+            wb.add_norm(n + '.norm', P)
             wq, wk, wv = (P(f'{n}.{t}.weight').reshape(c, c) for t in 'qkv')
-            add_conv(n + '.qk', torch.cat([wq, wk]).reshape(2 * c, c, 1, 1), bias=torch.cat([P(n + '.q.bias'), P(n + '.k.bias')]))
+            wb.add_gemm(n + '.qk', torch.cat([wq, wk]).reshape(2 * c, c, 1, 1), bias=torch.cat([P(n + '.q.bias'), P(n + '.k.bias')]))
             wb.add(n + '.v:w', G.split_planes(wv))                       # [2][C][C]: the M operand of the V^T GEMM
             wb.add(n + '.v:b', P(n + '.v.bias'))
-            add_conv(n + '.proj', P(n + '.proj_out.weight'), bias=P(n + '.proj_out.bias'))
+            wb.add_gemm(n + '.proj', P(n + '.proj_out.weight'), bias=P(n + '.proj_out.bias'))
         elif m[0] == 'up':
-            add_conv(n, P(n + '.conv.weight'), bias=P(n + '.conv.bias'))
-    add_norm('norm_out', 'decoder.norm_out')
-    add_conv('conv_out', P('decoder.conv_out.weight'), bias=P('decoder.conv_out.bias'))
+            wb.add_gemm(n, P(n + '.conv.weight'), bias=P(n + '.conv.bias'))
+    wb.add_norm('norm_out', P, 'decoder.norm_out')
+    wb.add_gemm('conv_out', P('decoder.conv_out.weight'), bias=P('decoder.conv_out.bias'))
     return wb
 
 
 def compile_vae_plan(mods, meta, wb, B, R, npass=3):
     """Lower the decoder for B latents of resolution R x R."""
-    A = _Arena()
-    ops = []
-    npl = 2
-    io = lambda slot: S.ref(S.SPACE_IO, slot)
-    W = wb.ref
-    tag = [0]
-    emit = lambda b: ops.append((tag[0], b))
-    n_gn = sum(2 if m[0] == 'res' else (1 if m[0] == 'attn' else 0) for m in mods) + 1
-    A.need('stats', n_gn * B * 32 * 2 * 8)
-    stat_i = [0]
+    pb = PlanBuilder(wb, B, npass)
+    emit, W = pb.emit, wb.ref
+    pb.stats(sum(2 if m[0] == 'res' else (1 if m[0] == 'attn' else 0) for m in mods) + 1)
 
-    def stats_slot():
-        i = stat_i[0]
-        stat_i[0] += 1
-        return i * B * 32 * 2 * 8
-
-    emit(lambda R_: S.MemsetDesc(ptr=R_('stats'), bytes=n_gn * B * 32 * 2 * 8))
-
-    def gn(src, c, H, g, b, silu, out, raw=None):
+    def gn(src, c, H, norm, silu, out, raw=None):
         """GroupNorm(32, eps 1e-6) (+ swish) of the fp32 NHWC tensor `src` -> fp16 planes `out` (+ raw planes for a 1x1 skip)."""
-        s = stats_slot()
-        emit(lambda R_: S.GnStatsDesc(src0=R_(src), src1=0, C0=c, C1=0, HW=H * H, B=B, groups=32, sums=R_('stats', s)))
-        emit(lambda R_: S.GnApplyDesc(src0=R_(src), src1=0, C0=c, C1=0, H=H, W=H, B=B, groups=32, sums=R_('stats', s), gamma=W(g), beta=W(b),
-                                      eps=1e-6, silu=silu, ada=0, ada_stride=0, resample=0, nplanes=npl, out_act=R_(out),
-                                      out_raw=R_(raw) if raw else 0, out_raw_f32=0))
+        pb.group_norm([(src, c)], H, norm, 1e-6, out, silu=silu, raw=raw)
 
     def lower_res(m, src, H):
         _, n, cin, cout = m
         M = B * H * H
         has_skip = cin != cout
-        A.need('act', npl * M * max(cin, cout) * H2)
+        pb.need('act', NPL * M * max(cin, cout) * H2)
         if has_skip:
-            A.need('raw', npl * M * cin * H2)
-        gn(src, cin, H, n + '.n1:g', n + '.n1:b', 1, 'act', raw='raw' if has_skip else None)
-        A.need('y', M * cout * F4)
+            pb.need('raw', NPL * M * cin * H2)
+        gn(src, cin, H, n + '.n1', 1, 'act', raw='raw' if has_skip else None)
+        pb.need('y', M * cout * F4)
         emit(lambda R_: G.conv_gemm(R_('act'), B, H, H, cin, W(n + '.c1:w'), cout, taps=9, npass=npass, out_f32=R_('y'), bias=W(n + '.c1:b'))[0])
-        gn('y', cout, H, n + '.n2:g', n + '.n2:b', 1, 'act')
-        out = A.need('h:' + n, M * cout * F4)
+        gn('y', cout, H, n + '.n2', 1, 'act')
+        out = pb.need('h:' + n, M * cout * F4)
         emit(lambda R_: G.conv_gemm(R_('act'), B, H, H, cout, W(n + '.c2:w'), cout, taps=9, npass=npass, a2_ptr=R_('raw') if has_skip else 0,
                                     C2=cin if has_skip else 0, out_f32=R_(out), bias=W(n + '.c2:b'), residual=0 if has_skip else R_(src),
                                     ldr=cout)[0])
@@ -148,24 +119,15 @@ def compile_vae_plan(mods, meta, wb, B, R, npass=3):
         L = H * H
         M = B * L
         assert L % 64 == 0, 'attention needs a multiple of 64 positions (K extent of the PV product)'
-        A.need('act', npl * M * c * H2)
-        gn(src, c, H, n + '.norm:g', n + '.norm:b', 0, 'act')
-        A.need('qk', npl * M * 2 * c * H2)
-        A.need('vt', npl * B * c * L * H2)
-        A.need('S', B * L * L * F4)
-        A.need('P', npl * B * L * L * H2)
-        A.need('o', npl * M * c * H2)
+        pb.need('act', NPL * M * c * H2)
+        gn(src, c, H, n + '.norm', 0, 'act')
+        pb.need('qk', NPL * M * 2 * c * H2)
+        pb.need('vt', NPL * B * c * L * H2)
         emit(lambda R_: G.conv_gemm(R_('act'), B, H, H, c, W(n + '.qk:w'), 2 * c, taps=1, npass=npass, out_h16=R_('qk'), bias=W(n + '.qk:b'))[0])
-        emit(lambda R_: G.rows_gemm(W(n + '.v:w'), c, c, 1, R_('act'), L, c, B, c, num_z=B, nh=1, m_valid=c, n_valid=L, npass=npass,
-                                    b_z_per_zb=1, out_h16=R_('vt'), o_zb=c * L, ldo=L, o_plane=B * c * L, bias_m=W(n + '.v:b'))[0])
-        emit(lambda R_: G.rows_gemm(R_('qk'), L, 2 * c, B, R_('qk'), L, 2 * c, B, c, num_z=B, nh=1, m_valid=L, n_valid=L, npass=npass,
-                                    a_c_per_zh=c, a_n_per_zb=1, b_k0=c, b_k_per_zh=c, b_z_per_zb=1, out_f32=R_('S'), o_zb=L * L, o_zh=L * L,
-                                    ldo=L, scale=float(c) ** -0.5)[0])
-        emit(lambda R_: S.SoftmaxDesc(S=R_('S'), P=R_('P'), rows=B * L, L=L, nplanes=npl, pitch_in=0, pitch_out=0))
-        emit(lambda R_: G.rows_gemm(R_('P'), L, L, B, R_('vt'), c, L, B, L, num_z=B, nh=1, m_valid=L, n_valid=c, npass=npass,
-                                    a_n_per_zb=1, a_n_per_zh=1, b_row_per_zh=c, b_z_per_zb=1, out_h16=R_('o'), o_zb=L * c, o_zh=c, ldo=c,
-                                    o_plane=M * c)[0])
-        out = A.need('h:' + n, M * c * F4)
+        pb.vt_gemm(n + '.v:w', 'act', c, c, L, L, bias=n + '.v:b')
+        pb.attention(False, 'qk', 'qk', 'o', 1, L, L, c, float(c) ** -0.5, L)
+        pb.need('o', NPL * M * c * H2)
+        out = pb.need('h:' + n, M * c * F4)
         emit(lambda R_: G.conv_gemm(R_('o'), B, H, H, c, W(n + '.proj:w'), c, taps=1, npass=npass, out_f32=R_(out), bias=W(n + '.proj:b'),
                                     residual=R_(src), ldr=c)[0])
         return out, c
@@ -173,27 +135,26 @@ def compile_vae_plan(mods, meta, wb, B, R, npass=3):
     def lower_up(m, src, H):
         _, n, c = m
         Ho = 2 * H
-        A.need('act', npl * B * Ho * Ho * c * H2)
-        emit(lambda R_: S.GnApplyDesc(src0=R_(src), src1=0, C0=c, C1=0, H=H, W=H, B=B, groups=32, sums=0, gamma=0, beta=0, eps=0.0, silu=0,
-                                      ada=0, ada_stride=0, resample=2, nplanes=npl, out_act=0, out_raw=R_('act'), out_raw_f32=0))
-        out = A.need('h:' + n, B * Ho * Ho * c * F4)
+        pb.need('act', NPL * B * Ho * Ho * c * H2)
+        pb.to_planes(src, c, H, H, B, 'act', resample=2)
+        out = pb.need('h:' + n, B * Ho * Ho * c * F4)
         emit(lambda R_: G.conv_gemm(R_('act'), B, Ho, Ho, c, W(n + ':w'), c, taps=9, npass=npass, out_f32=R_(out), bias=W(n + ':b'))[0])
         return out, c, Ho
 
     # ---- z / scale_factor -> fp16 planes (channels zero-padded to 64) -> post_quant_conv (1x1) -> conv_in (3x3) -------------------------
     HW = R * R
-    A.need('in_planes', npl * B * HW * 64 * H2)
-    emit(lambda R_: S.PrepInputDesc(x=io(S.DS_IO_X), coef=io(S.DS_IO_LABELS), coef_stride=0, B=B, C=meta['embed_dim'], HW=HW, nplanes=npl,
+    pb.need('in_planes', NPL * B * HW * 64 * H2)
+    emit(lambda R_: S.PrepInputDesc(x=io(S.DS_IO_X), coef=io(S.DS_IO_LABELS), coef_stride=0, B=B, C=meta['embed_dim'], HW=HW, nplanes=NPL,
                                     x_batch=B, out=R_('in_planes')))
     # dedicated buffer: only z_channels of its 64 columns are ever written, the rest stay at the arena's initial zeros
-    A.need('pq_planes', npl * B * HW * 64 * H2)
+    pb.need('pq_planes', NPL * B * HW * 64 * H2)
     emit(lambda R_: G.conv_gemm(R_('in_planes'), B, R, R, 64, W('post_quant_conv:w'), meta['z_channels'], taps=1, npass=npass,
                                 out_h16=R_('pq_planes'), ldo=64, bias=W('post_quant_conv:b'))[0])
     cur, cur_c, H = None, None, R
     for m in mods:
-        tag[0] += 1
+        pb.tag += 1
         if m[0] == 'conv':
-            cur = A.need('h:' + m[1], B * HW * m[3] * F4)
+            cur = pb.need('h:' + m[1], B * HW * m[3] * F4)
             emit(lambda R_, m=m, cur=cur: G.conv_gemm(R_('pq_planes'), B, R, R, 64, W(m[1] + ':w'), m[3], taps=9, npass=npass, out_f32=R_(cur),
                                                       bias=W(m[1] + ':b'))[0])
             cur_c = m[3]
@@ -204,22 +165,11 @@ def compile_vae_plan(mods, meta, wb, B, R, npass=3):
         elif m[0] == 'up':
             cur, cur_c, H = lower_up(m, cur, H)
     # ---- norm_out + swish + conv_out -> images, NCHW fp32 ----------------------------------------------------------------------------
-    tag[0] += 1
-    A.need('act', npl * B * H * H * cur_c * H2)
-    gn(cur, cur_c, H, 'norm_out:g', 'norm_out:b', 1, 'act')
+    pb.tag += 1
+    pb.need('act', NPL * B * H * H * cur_c * H2)
+    gn(cur, cur_c, H, 'norm_out', 1, 'act')
     fin_c, fin_H = cur_c, H
     emit(lambda R_: G.conv_gemm(R_('act'), B, fin_H, fin_H, fin_c, W('conv_out:w'), meta['out_ch'], taps=9, npass=npass, bias=W('conv_out:b'),
-                                edm=(0, 0, 0, meta['out_ch'], io(S.DS_IO_D)))[0])
-    assert stat_i[0] <= n_gn and H == R * meta['upscale']
-
-    total = A.finalize()
-    arr = (S.PlanOp * len(ops))()
-    for i, (tg, builder) in enumerate(ops):
-        desc = builder(A.ref)
-        if isinstance(desc, S.GemmDesc) and desc.edm_out == 1 and desc.edm_x == 0:
-            desc.edm_out = 2                       # plain NCHW fp32 write of the epilogue value
-        arr[i].type = S.OP_TYPE_OF[type(desc)]
-        arr[i].tag = tg
-        setattr(arr[i].u, S.UNION_FIELD[arr[i].type], desc)
-    plan_meta = dict(B=B, R=R, out_res=H, npass=npass, n_ops=len(ops), n_gemm=sum(1 for i in range(len(ops)) if arr[i].type == S.DS_OP_GEMM))
-    return Plan(arr, len(ops), total, dict(A.offsets), plan_meta)
+                                nchw_out=(meta['out_ch'], io(S.DS_IO_D)))[0])
+    assert H == R * meta['upscale']
+    return pb.finish(B=B, R=R, out_res=H, npass=npass)
