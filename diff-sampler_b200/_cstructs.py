@@ -66,7 +66,7 @@ class LinearDesc(C.Structure):
 
 class PrepInputDesc(C.Structure):
     _fields_ = [('x', P), ('coef', P), ('coef_stride', I32), ('B', I32), ('C', I32), ('HW', I32), ('nplanes', I32),
-                ('x_batch', I32), ('out', P)]
+                ('x_batch', I32), ('out', P), ('codebook', P), ('idx', P), ('n_embed', I32), ('pad0', I32)]
 
 
 class ChanmeanDesc(C.Structure):

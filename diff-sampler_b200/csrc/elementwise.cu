@@ -708,6 +708,72 @@ __global__ void prep_input_kernel(ds_prep_input_desc d) {
     if (d.nplanes > 1) *reinterpret_cast<uint4*>(o + (long long)d.B * d.HW * 64 + off) = *reinterpret_cast<const uint4*>(lo);
 }
 
+// Vector-quantized input: one thread per pixel holds v = c_in * x (channels zero-padded to CP) and streams the codebook through shared
+// memory in chunks of VQ_CHUNK rows; the padded channels are zero on both sides, so they add exactly 0 to every distance.  A strict
+// '<' over ascending rows keeps the lowest index among equal distances (torch.argmin).  The chosen row is then written, split hi/lo,
+// into the 64-column planes prep_input_kernel writes.
+constexpr int VQ_CHUNK = 1024;
+
+template <int CP>
+__global__ void __launch_bounds__(256) vq_prep_input_kernel(ds_prep_input_desc d) {
+    __shared__ float4 s_code[VQ_CHUNK * (CP / 4)];
+    const long long px = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total = (long long)d.B * d.HW;
+    const bool live = px < total;
+    const int n = live ? (int)(px / d.HW) : 0;
+    const int hw = live ? (int)(px - (long long)n * d.HW) : 0;
+    const int xb = d.x_batch > 0 ? d.x_batch : d.B;
+    const int nx = n % xb;
+    float v[CP];
+    if (live) {
+        const float cin = d.coef[nx * d.coef_stride + 2];
+#pragma unroll
+        for (int c = 0; c < CP; ++c) v[c] = c < d.C ? cin * d.x[((long long)nx * d.C + c) * d.HW + hw] : 0.f;
+    }
+    float best = INFINITY;
+    int bi = 0;
+    float* sc = reinterpret_cast<float*>(s_code);
+    for (int base = 0; base < d.n_embed; base += VQ_CHUNK) {
+        const int cnt = min(VQ_CHUNK, d.n_embed - base);
+        __syncthreads();
+        for (int i = threadIdx.x; i < cnt * CP; i += blockDim.x) {
+            const int j = i / CP, c = i - j * CP;
+            sc[i] = c < d.C ? d.codebook[(long long)(base + j) * d.C + c] : 0.f;
+        }
+        __syncthreads();
+        if (!live) continue;
+        for (int j = 0; j < cnt; ++j) {
+            float dist = 0.f;
+#pragma unroll
+            for (int q = 0; q < CP / 4; ++q) {
+                const float4 e = s_code[j * (CP / 4) + q];
+                const float d0 = v[4 * q] - e.x, d1 = v[4 * q + 1] - e.y, d2 = v[4 * q + 2] - e.z, d3 = v[4 * q + 3] - e.w;
+                dist = fmaf(d0, d0, dist);
+                dist = fmaf(d1, d1, dist);
+                dist = fmaf(d2, d2, dist);
+                dist = fmaf(d3, d3, dist);
+            }
+            if (dist < best) { best = dist; bi = base + j; }
+        }
+    }
+    if (!live) return;
+    if (d.idx) d.idx[px] = bi;
+    __half* o = reinterpret_cast<__half*>(d.out);
+    const long long plane = total * 64;
+#pragma unroll
+    for (int c8 = 0; c8 < 8; ++c8) {
+        __align__(16) __half hi[8];
+        __align__(16) __half lo[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = c8 * 8 + j;
+            split_h16(c < d.C ? d.codebook[(long long)bi * d.C + c] : 0.f, hi[j], lo[j]);
+        }
+        *reinterpret_cast<uint4*>(o + px * 64 + c8 * 8) = *reinterpret_cast<const uint4*>(hi);
+        if (d.nplanes > 1) *reinterpret_cast<uint4*>(o + plane + px * 64 + c8 * 8) = *reinterpret_cast<const uint4*>(lo);
+    }
+}
+
 // one warp per token row; the row lives in registers (C <= 2048), two-pass mean / variance like torch's layer_norm
 __global__ void layernorm_kernel(ds_layernorm_desc d) {
     const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -1086,6 +1152,13 @@ extern "C" int ds_linear_launch(const ds_linear_desc* d, cudaStream_t stream) {
 
 extern "C" int ds_prep_input_launch(const ds_prep_input_desc* d, cudaStream_t stream) {
     if (d->C > 64) return -2;
+    if (d->codebook) {
+        if (d->C > 8 || d->n_embed < 1) return -2;
+        const unsigned blocks = (unsigned)(((long long)d->B * d->HW + 255) / 256);
+        if (d->C <= 4) vq_prep_input_kernel<4><<<blocks, 256, 0, stream>>>(*d);
+        else vq_prep_input_kernel<8><<<blocks, 256, 0, stream>>>(*d);
+        return ok();
+    }
     const long long total = (long long)d->B * d->HW * 8;
     prep_input_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(*d);
     return ok();

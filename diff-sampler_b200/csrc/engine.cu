@@ -91,7 +91,7 @@ static void visit_ptrs(ds_plan_op& op, F f) {
         case DS_OP_SOFTMAX: { auto& d = op.u.softmax; P(d.S); P(d.P); break; }
         case DS_OP_POSEMB: { auto& d = op.u.posemb; P(d.sigma); P(d.coef); P(d.emb); break; }
         case DS_OP_LINEAR: { auto& d = op.u.linear; P(d.in); P(d.W); P(d.b); P(d.add); P(d.out); break; }
-        case DS_OP_PREP_INPUT: { auto& d = op.u.prep_input; P(d.x); P(d.coef); P(d.out); break; }
+        case DS_OP_PREP_INPUT: { auto& d = op.u.prep_input; P(d.x); P(d.coef); P(d.out); P(d.codebook); P(d.idx); break; }
         case DS_OP_CHANMEAN: { auto& d = op.u.chanmean; P(d.src); P(d.out); break; }
         case DS_OP_MEMSET: { auto& d = op.u.memset; P(d.ptr); break; }
         case DS_OP_LAYERNORM: { auto& d = op.u.layernorm; P(d.src); P(d.gamma); P(d.beta); P(d.out); break; }

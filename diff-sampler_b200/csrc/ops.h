@@ -229,6 +229,9 @@ typedef struct ds_linear_desc {
 
 // Network input: x (NCHW fp32) * c_in[n] -> fp16 planes NHWC with channels zero-padded to 64.
 // Reference: networks_edm.py:493 (c_in * x).
+// With `codebook` set (first stage of a VQ autoencoder, VQModelInterface.decode -> VectorQuantizer2, autoencoder.py:274-282), each
+// pixel's C-vector v = c_in * x is first replaced by its nearest codebook row: argmin_j sum_c (v_c - e_jc)^2 in fp32, ties to the lowest
+// j as torch.argmin.  C <= 8 then.
 typedef struct ds_prep_input_desc {
     const float* x;
     const float* coef;      // from ds_posemb_desc
@@ -237,6 +240,10 @@ typedef struct ds_prep_input_desc {
     int32_t nplanes;
     int32_t x_batch;        // 0 or B: batch of x; sample n reads x[n % x_batch] (classifier-free guidance evaluates [x, x])
     void* out;              // fp16 [nplanes][B][HW][64]
+    const float* codebook;  // [n_embed][C] fp32, or NULL (no quantization)
+    int32_t* idx;           // [B][HW] chosen codebook rows (debug read-out), or NULL
+    int32_t n_embed;
+    int32_t pad0;
 } ds_prep_input_desc;
 
 // LayerNorm over the last dim of fp32 [rows][C] -> fp16 hi/lo planes (LDM BasicTransformerBlock.norm1/2/3, attention.py:203-215).

@@ -10,6 +10,11 @@ wgmma GEMM kernel for every convolution (1x1 skip `nin_shortcut` appended along 
 wide-head attention, the row softmax.  New for this net: image rows wider than one 128-pixel M tile (256- and 512-wide levels) --
 `gemm_desc.conv_gemm` then tiles them as 128-pixel row segments.
 io slots: X = latents [B, z_ch, R, R] (NCHW fp32), LABELS = coef [1][4] with 1/scale_factor in slot 2, D = images [B, out_ch, sR, sR].
+
+VQ first stages (`VQModelInterface.decode`, autoencoder.py:274-282, e.g. the VQ-f4 of the LSUN-Bedroom / FFHQ LDMs) differ only in
+front: the state dict also holds `quantize.embedding.weight` [n_embed, embed_dim], and unless the caller passes force_not_quantize the
+input op snaps every latent pixel to its nearest codebook row (VectorQuantizer2 inference: argmin of the squared L2 distance, then that
+row) while it writes post_quant_conv's operand planes (csrc/elementwise.cu vq_prep_input_kernel).
 """
 from collections import OrderedDict
 
@@ -21,12 +26,13 @@ from .plan import F4, H2, NPL, PlanBuilder, WeightBlob, io
 
 
 def vae_structure(params):
-    """Execution-ordered module list from `first_stage_model.state_dict()` names / shapes (decoder.* and post_quant_conv.*):
-    [('conv', name, cin, cout) | ('res', name, cin, cout) | ('attn', name, c) | ('up', name, c)], meta."""
+    """Execution-ordered module list from `first_stage_model.state_dict()` names / shapes (decoder.*, post_quant_conv.* and, for a VQ
+    first stage, quantize.embedding.weight):
+    [('conv', name, cin, cout) | ('res', name, cin, cout) | ('attn', name, c) | ('up', name, c)], meta (+ n_embed for a VQ first stage)."""
     def shp(k):
         return tuple(params[k].shape)
     P = params
-    assert 'decoder.conv_in.weight' in P and 'post_quant_conv.weight' in P, 'not an AutoencoderKL decoder state_dict'
+    assert 'decoder.conv_in.weight' in P and 'post_quant_conv.weight' in P, 'not an AutoencoderKL / VQModel decoder state_dict'
     block_in = shp('decoder.conv_in.weight')[0]
     mods = [('conv', 'decoder.conv_in', shp('decoder.conv_in.weight')[1], block_in)]
     for n in ('decoder.mid.block_1', 'decoder.mid.attn_1', 'decoder.mid.block_2'):
@@ -50,6 +56,12 @@ def vae_structure(params):
     for m in mods:
         for c in m[2:]:
             assert m[0] == 'conv' or c % 64 == 0, f'{m[1]}: channel counts must be multiples of 64, got {c}'
+    if 'quantize.embedding.weight' in P:                          # VQModelInterface: latents are snapped to a codebook row first
+        n_embed, e_dim = shp('quantize.embedding.weight')
+        if e_dim != meta['embed_dim'] or e_dim > 8:
+            raise ValueError(f'quantize.embedding.weight {(n_embed, e_dim)}: the codebook must have embed_dim = '
+                             f'{meta["embed_dim"]} <= 8 columns')
+        meta['n_embed'] = n_embed
     return mods, meta
 
 
@@ -84,11 +96,17 @@ def pack_vae_weights(mods, meta, params):
             wb.add_gemm(n, P(n + '.conv.weight'), bias=P(n + '.conv.bias'))
     wb.add_norm('norm_out', P, 'decoder.norm_out')
     wb.add_gemm('conv_out', P('decoder.conv_out.weight'), bias=P('decoder.conv_out.bias'))
+    if 'n_embed' in meta:
+        wb.add('quantize:e', P('quantize.embedding.weight'))          # fp32 [n_embed][embed_dim]
     return wb
 
 
-def compile_vae_plan(mods, meta, wb, B, R, npass=3):
-    """Lower the decoder for B latents of resolution R x R."""
+def compile_vae_plan(mods, meta, wb, B, R, npass=3, quantize=False, debug_indices=False):
+    """Lower the decoder for B latents of resolution R x R.  quantize (VQ first stages only): snap each latent pixel to its nearest
+    codebook row before post_quant_conv, as VQModelInterface.decode does unless force_not_quantize; debug_indices then also keeps the
+    chosen rows in the int32 arena buffer 'vq_idx' [B][R * R]."""
+    if quantize and 'n_embed' not in meta:
+        raise ValueError('quantize: this first stage has no codebook (not a VQModelInterface)')
     pb = PlanBuilder(wb, B, npass)
     emit, W = pb.emit, wb.ref
     pb.stats(sum(2 if m[0] == 'res' else (1 if m[0] == 'attn' else 0) for m in mods) + 1)
@@ -141,11 +159,14 @@ def compile_vae_plan(mods, meta, wb, B, R, npass=3):
         emit(lambda R_: G.conv_gemm(R_('act'), B, Ho, Ho, c, W(n + ':w'), c, taps=9, npass=npass, out_f32=R_(out), bias=W(n + ':b'))[0])
         return out, c, Ho
 
-    # ---- z / scale_factor -> fp16 planes (channels zero-padded to 64) -> post_quant_conv (1x1) -> conv_in (3x3) -------------------------
+    # ---- z / scale_factor (-> nearest codebook row) -> fp16 planes (channels zero-padded to 64) -> post_quant_conv (1x1) -> conv_in ------
     HW = R * R
     pb.need('in_planes', NPL * B * HW * 64 * H2)
+    vq = {}
+    if quantize:
+        vq = dict(codebook=W('quantize:e'), n_embed=meta['n_embed'])
     emit(lambda R_: S.PrepInputDesc(x=io(S.DS_IO_X), coef=io(S.DS_IO_LABELS), coef_stride=0, B=B, C=meta['embed_dim'], HW=HW, nplanes=NPL,
-                                    x_batch=B, out=R_('in_planes')))
+                                    x_batch=B, out=R_('in_planes'), idx=R_('vq_idx') if quantize and debug_indices else 0, **vq))
     # dedicated buffer: only z_channels of its 64 columns are ever written, the rest stay at the arena's initial zeros
     pb.need('pq_planes', NPL * B * HW * 64 * H2)
     emit(lambda R_: G.conv_gemm(R_('in_planes'), B, R, R, 64, W('post_quant_conv:w'), meta['z_channels'], taps=1, npass=npass,
@@ -172,4 +193,6 @@ def compile_vae_plan(mods, meta, wb, B, R, npass=3):
     emit(lambda R_: G.conv_gemm(R_('act'), B, fin_H, fin_H, fin_c, W('conv_out:w'), meta['out_ch'], taps=9, npass=npass, bias=W('conv_out:b'),
                                 nchw_out=(meta['out_ch'], io(S.DS_IO_D)))[0])
     assert H == R * meta['upscale']
-    return pb.finish(B=B, R=R, out_res=H, npass=npass)
+    if quantize and debug_indices:
+        pb.need('vq_idx', B * HW * 4)                             # last: the other buffers keep the offsets of the plain plan
+    return pb.finish(B=B, R=R, out_res=H, npass=npass, **({'quantize': True} if quantize else {}))
