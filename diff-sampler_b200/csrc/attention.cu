@@ -14,6 +14,7 @@
 //
 // Same split-precision contract as the GEMM kernel: Q, K, V and P are fp16 hi + lo planes, products are hi*hi + lo*hi + hi*lo in fp32.
 #include "ops.h"
+#include "operand.cuh"
 #include "ptx.cuh"
 #include <cuda_fp16.h>
 #include <math.h>
@@ -53,14 +54,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-
-__device__ __forceinline__ void split_half2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    const __half2 h2 = __floats2half2_rn(a, b);
-    const float2 hf = __half22float2(h2);
-    const __half2 l2 = __floats2half2_rn(a - hf.x, b - hf.y);
-    hi = *reinterpret_cast<const uint32_t*>(&h2);
-    lo = *reinterpret_cast<const uint32_t*>(&l2);
 }
 
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_constant__ AttnKernelParams p) {
@@ -174,7 +167,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
             const float p0 = col < kv[hr] ? ex2_approx(fmaf(S[i], p.scale_log2e, -mn[hr])) : 0.f;
             const float p1 = col + 1 < kv[hr] ? ex2_approx(fmaf(S[i + 1], p.scale_log2e, -mn[hr])) : 0.f;
             ls[hr] += p0 + p1;
-            split_half2(p0, p1, Ph[i >> 1], Pl[i >> 1]);
+            split_h16_pair(p0, p1, Ph[i >> 1], Pl[i >> 1]);
         }
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
@@ -219,10 +212,8 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
         __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * 64 + 2 * (lane & 3);
 #pragma unroll
         for (int g = 0; g < 8; ++g) {
-            uint32_t hi, lo;
-            split_half2(O[4 * g + 2 * hr] * inv, O[4 * g + 2 * hr + 1] * inv, hi, lo);
-            *reinterpret_cast<uint32_t*>(o + 8 * g) = hi;
-            *reinterpret_cast<uint32_t*>(o + p.o_plane + 8 * g) = lo;
+            const float v[2] = {O[4 * g + 2 * hr] * inv, O[4 * g + 2 * hr + 1] * inv};
+            store_planes<2>(o, p.o_plane, 8 * g, v, 2);
         }
     }
 }

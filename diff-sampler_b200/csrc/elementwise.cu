@@ -1,19 +1,13 @@
 // HBM-bound companions of the tensor-core kernels: GroupNorm statistics / apply (+SiLU, +resample),
 // row softmax, timestep embedding, small dense layers, input preparation.  All NHWC, 128-bit accesses.
 #include "ops.h"
+#include "operand.cuh"
 #include <cuda_fp16.h>
-#include <cuda_fp8.h>
 #include <math.h>
-#include <stdlib.h>
 
 namespace dsb {
 
 __device__ __forceinline__ float silu_f(float v) { return __fdividef(v, 1.0f + __expf(-v)); }
-
-__device__ __forceinline__ void split_h16(float v, __half& hi, __half& lo) {
-    hi = __float2half_rn(v);
-    lo = __float2half_rn(v - __half2float(hi));
-}
 
 // ------------------------------------------------------------------------------------------ GN stats
 // grid (chunks, B); block (ncol4 <= 384, rows).  Thread (tx, ty) owns float4 column tx.
@@ -62,6 +56,36 @@ __global__ void gn_stats_kernel(ds_gn_stats_desc d, int pix_per_cta) {
         atomicAdd(&d.sums[((long long)n * d.groups + tid) * 2 + 0], s_sum[tid]);
         atomicAdd(&d.sums[((long long)n * d.groups + tid) * 2 + 1], s_sq[tid]);
     }
+}
+
+// ------------------------------------------------------------------------------------------ GN coefficients
+// {mean, 1 / sqrt(var + eps)} of group g of sample n, from its fp64 {sum, sum of squares} over cnt values (D: the apply or finalize
+// descriptor).
+template <class D>
+__device__ __forceinline__ float2 gn_group_stats(const D& d, int n, int g, double cnt) {
+    const double s = d.sums[((long long)n * d.groups + g) * 2 + 0];
+    const double q = d.sums[((long long)n * d.groups + g) * 2 + 1];
+    const double mu = s / cnt;
+    double var = q / cnt - mu * mu;
+    if (var < 0.0) var = 0.0;
+    const float rstd = (float)(1.0 / sqrt(var + (double)d.eps));
+    return make_float2((float)mu, rstd);
+}
+
+// Channel c + j of sample n normalises as y = (x - mean) * a + b: a = rstd * gamma * (1 + ada_scale), b = beta * (1 + ada_scale) +
+// ada_shift.
+template <class D>
+__device__ __forceinline__ void gn_channel_coef(const D& d, int n, int C, int c, int j, float rstd, float& a, float& b) {
+    float aa = rstd * __ldg(d.gamma + c + j);
+    float bb = __ldg(d.beta + c + j);
+    if (d.ada) {
+        const float sc = d.ada[(long long)n * d.ada_stride + c + j] + 1.0f;
+        const float sh = d.ada[(long long)n * d.ada_stride + C + c + j];
+        aa *= sc;
+        bb = bb * sc + sh;
+    }
+    a = aa;
+    b = bb;
 }
 
 // ------------------------------------------------------------------------------------------ GN statistics from quad partials
@@ -120,26 +144,16 @@ __global__ void __launch_bounds__(1024) gn_finalize_kernel(ds_gn_finalize_desc d
     // second product: y = x * a + b per (sample, channel), so that gn_apply starts streaming without an fp64 prologue per thread
     const double cnt = (double)(C / d.groups) * d.HW;
     for (int g = threadIdx.x; g < d.groups; g += blockDim.x) {
-        const double s = d.sums[((long long)n * d.groups + g) * 2 + 0];
-        const double q = d.sums[((long long)n * d.groups + g) * 2 + 1];
-        const double mu = s / cnt;
-        double var = q / cnt - mu * mu;
-        if (var < 0.0) var = 0.0;
-        s_mu[g] = (float)mu;
-        s_rstd[g] = (float)(1.0 / sqrt(var + (double)d.eps));
+        const float2 st = gn_group_stats(d, n, g, cnt);
+        s_mu[g] = st.x;
+        s_rstd[g] = st.y;
     }
     __syncthreads();
     const int cpg = C / d.groups;
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
         const int g = c / cpg;
-        float aa = s_rstd[g] * __ldg(d.gamma + c);
-        float bb = __ldg(d.beta + c);
-        if (d.ada) {
-            const float sc = d.ada[(long long)n * d.ada_stride + c] + 1.0f;
-            const float sh = d.ada[(long long)n * d.ada_stride + C + c];
-            aa *= sc;
-            bb = bb * sc + sh;
-        }
+        float aa, bb;
+        gn_channel_coef(d, n, C, c, 0, s_rstd[g], aa, bb);
         reinterpret_cast<float2*>(d.coef)[(long long)n * C + c] = make_float2(aa, fmaf(-s_mu[g], aa, bb));
     }
 }
@@ -147,57 +161,7 @@ __global__ void __launch_bounds__(1024) gn_finalize_kernel(ds_gn_finalize_desc d
 // ------------------------------------------------------------------------------------------ GN apply
 // grid (chunks, B); block = nc8 * rows threads.  Thread (c8, prow) owns 8 fixed channels: its normalisation coefficients
 // live in registers (mean, a = rstd*gamma*(1+ada_scale), b = beta*(1+ada_scale)+ada_shift) and it streams over output pixels.
-// fmt 1 (operand of an f8 GEMM, csrc/ops.h): fp16 plane of v * 2^A16 (saturating) followed by the two e4m3 byte planes
-// (v - hi) * 2^LO8 and hi * 2^HI8, where hi is the value the fp16 plane represents.  Powers of two: the roundings are those of v.
-// Packed arithmetic (two values per instruction wherever the ISA has it): v * 2^A16 -> f16x2 convert -> clamp as half2 (a value beyond the fp16
-// range converts to inf and is clamped back: the same result as clamping first) -> hi byte plane straight from the half2
-// (cvt.e4m3x2.f16x2 of hi * 2^(HI8 - A16), exact: a power of two) -> lo = fma(hi, -2^(LO8 - A16), v * 2^LO8) = (v - hi / 2^A16) * 2^LO8 with
-// one rounding.  7 instructions per value instead of 11 (gn_apply with this store is otherwise bound by instruction issue).
-__device__ __forceinline__ void f8_image_pair(float v0, float v1, uint32_t& hi16, unsigned short& lo8, unsigned short& hi8) {
-    constexpr float kA16 = (float)(1 << DS_F8_SH_A16), kLo8 = (float)(1 << DS_F8_SH_LO8);
-    constexpr float kLoA = (float)(1 << (DS_F8_SH_LO8 - DS_F8_SH_A16));
-    static_assert(DS_F8_SH_A16 >= DS_F8_SH_HI8 && DS_F8_SH_LO8 >= DS_F8_SH_A16, "operand scales");
-    const __half2 lim = __float2half2_rn(65504.f);
-    __half2 h = __floats2half2_rn(v0 * kA16, v1 * kA16);
-    h = __hmin2(__hmax2(h, __hneg2(lim)), lim);
-    hi16 = *reinterpret_cast<const uint32_t*>(&h);
-    const float2 hf = __half22float2(h);
-    lo8 = __nv_cvt_float2_to_fp8x2(make_float2(fmaf(hf.x, -kLoA, v0 * kLo8), fmaf(hf.y, -kLoA, v1 * kLo8)), __NV_SATFINITE, __NV_E4M3);
-    const __half2 h8 = __hmul2(h, __float2half2_rn(1.0f / (float)(1 << (DS_F8_SH_A16 - DS_F8_SH_HI8))));
-    hi8 = __nv_cvt_halfraw2_to_fp8x2(*reinterpret_cast<const __half2_raw*>(&h8), __NV_SATFINITE, __NV_E4M3);
-}
-
-__device__ __forceinline__ void gn_store_f8(__half* base, long long plane, long long o, const float* v) {
-    __align__(16) uint32_t hi[4];
-    __align__(8) unsigned short lo8[4];
-    __align__(8) unsigned short hi8[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) f8_image_pair(v[2 * j], v[2 * j + 1], hi[j], lo8[j], hi8[j]);
-    *reinterpret_cast<uint4*>(base + o) = *reinterpret_cast<const uint4*>(hi);
-    unsigned char* b8 = reinterpret_cast<unsigned char*>(base + plane);
-    *reinterpret_cast<uint2*>(b8 + o) = *reinterpret_cast<const uint2*>(lo8);
-    *reinterpret_cast<uint2*>(b8 + plane + o) = *reinterpret_cast<const uint2*>(hi8);
-}
-
-// fp16 hi / lo planes of two values: one packed convert each way (hi = rn(v), lo = rn(v - hi), as split_h16)
-__device__ __forceinline__ void split_h16_pair(float v0, float v1, uint32_t& hi, uint32_t& lo) {
-    const __half2 h = __floats2half2_rn(v0, v1);
-    const float2 hf = __half22float2(h);
-    const __half2 l = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
-    hi = *reinterpret_cast<const uint32_t*>(&h);
-    lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
-__device__ __forceinline__ void gn_store_planes(__half* base, long long plane, long long o, const float* v, int nplanes, int fmt = 0) {
-    if (fmt == 1) { gn_store_f8(base, plane, o, v); return; }
-    __align__(16) uint32_t hi[4];
-    __align__(16) uint32_t lo[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) split_h16_pair(v[2 * j], v[2 * j + 1], hi[j], lo[j]);
-    *reinterpret_cast<uint4*>(base + o) = *reinterpret_cast<const uint4*>(hi);
-    if (nplanes > 1) *reinterpret_cast<uint4*>(base + plane + o) = *reinterpret_cast<const uint4*>(lo);
-}
-
+// RESAMPLE 1 (2x2 mean), 2 (nearest x2) or 3 (space-to-depth); resample 0 runs gn_apply_v2_kernel / gn_apply_v3_kernel below.
 template <int RESAMPLE>
 __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int pix_per_cta, int nc8, int rows) {
     const int C = d.C0 + d.C1;
@@ -216,24 +180,13 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int p
         for (int j = 0; j < 8; ++j) {
             const int g = (c + j) / cpg;
             if (g != g_prev) {                 // at most a few distinct groups per 8 channels
-                const double s = d.sums[((long long)n * d.groups + g) * 2 + 0];
-                const double q = d.sums[((long long)n * d.groups + g) * 2 + 1];
-                const double mu = s / cnt;
-                double var = q / cnt - mu * mu;
-                if (var < 0.0) var = 0.0;
-                rstd = (float)(1.0 / sqrt(var + (double)d.eps));
-                mu_f = (float)mu;
+                const float2 st = gn_group_stats(d, n, g, cnt);
+                mu_f = st.x;
+                rstd = st.y;
                 g_prev = g;
             }
-            float aa = rstd * __ldg(d.gamma + c + j);
-            float bb = __ldg(d.beta + c + j);
-            if (d.ada) {
-                const float sc = d.ada[(long long)n * d.ada_stride + c + j] + 1.0f;
-                const float sh = d.ada[(long long)n * d.ada_stride + C + c + j];
-                aa *= sc;
-                bb = bb * sc + sh;
-            }
-            mean[j] = mu_f; a[j] = aa; b[j] = bb;
+            gn_channel_coef(d, n, C, c, j, rstd, a[j], b[j]);
+            mean[j] = mu_f;
         }
     }
     const int Ho = RESAMPLE == 1 ? d.H / 2 : (RESAMPLE == 2 ? d.H * 2 : d.H);
@@ -250,42 +203,7 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int p
     const int p_begin = blockIdx.x * pix_per_cta;
     int p_end = p_begin + pix_per_cta;
     if (p_end > npix) p_end = npix;
-    int p_begin_tail = p_begin + prow;
-    if (RESAMPLE == 0) {
-        // plain path (the common case): two pixels per iteration so that four 16-byte loads are in flight per thread
-        int po = p_begin + prow;
-        for (; po + rows < p_end; po += 2 * rows) {
-            const float* s0 = base + (long long)po * pitch;
-            const float* s1 = base + (long long)(po + rows) * pitch;
-            const float4 a0 = __ldcs(reinterpret_cast<const float4*>(s0));
-            const float4 a1 = __ldcs(reinterpret_cast<const float4*>(s0) + 1);
-            const float4 b0 = __ldcs(reinterpret_cast<const float4*>(s1));
-            const float4 b1 = __ldcs(reinterpret_cast<const float4*>(s1) + 1);
-            const float ea[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            const float eb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-            float ya[8], yb[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float u = 0.f, w = 0.f;
-                if (norm) {
-                    u = (ea[j] - mean[j]) * a[j] + b[j];
-                    w = (eb[j] - mean[j]) * a[j] + b[j];
-                    if (d.silu) { u = silu_f(u); w = silu_f(w); }
-                }
-                ya[j] = u; yb[j] = w;
-            }
-            const long long oa = ((long long)n * npix + po) * C + c;
-            const long long ob = ((long long)n * npix + po + rows) * C + c;
-            if (oact) { gn_store_planes(oact, plane, oa, ya, d.nplanes, d.fmt); gn_store_planes(oact, plane, ob, yb, d.nplanes, d.fmt); }
-            if (oraw) { gn_store_planes(oraw, plane, oa, ea, d.nplanes, d.fmt); gn_store_planes(oraw, plane, ob, eb, d.nplanes, d.fmt); }
-            if (d.out_raw_f32) {
-                *reinterpret_cast<float4*>(d.out_raw_f32 + oa) = a0; *reinterpret_cast<float4*>(d.out_raw_f32 + oa + 4) = a1;
-                *reinterpret_cast<float4*>(d.out_raw_f32 + ob) = b0; *reinterpret_cast<float4*>(d.out_raw_f32 + ob + 4) = b1;
-            }
-        }
-        p_begin_tail = po;
-    }
-    for (int po = (RESAMPLE == 0 ? p_begin_tail : p_begin + prow); po < p_end; po += rows) {
+    for (int po = p_begin + prow; po < p_end; po += rows) {
         const int ho = po / Wo, wo = po - ho * Wo;
         float act[8], raw[8];
         if (RESAMPLE == 1) {
@@ -331,8 +249,8 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int p
             const int h2 = ho >> 1, w2 = wo >> 1, ph = ((ho & 1) << 1) | (wo & 1);
             o = (((long long)n * (d.H / 2) + h2) * (d.W / 2) + w2) * (4LL * C) + (long long)ph * C + c;
         }
-        if (oact) gn_store_planes(oact, plane, o, act, d.nplanes, d.fmt);
-        if (oraw) gn_store_planes(oraw, plane, o, raw, d.nplanes, d.fmt);
+        if (oact) store_operand<8>(oact, plane, o, act, d.nplanes, d.fmt);
+        if (oraw) store_operand<8>(oraw, plane, o, raw, d.nplanes, d.fmt);
         if (d.out_raw_f32) {
             *reinterpret_cast<float4*>(d.out_raw_f32 + o) = make_float4(raw[0], raw[1], raw[2], raw[3]);
             *reinterpret_cast<float4*>(d.out_raw_f32 + o + 4) = make_float4(raw[4], raw[5], raw[6], raw[7]);
@@ -340,10 +258,9 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int p
     }
 }
 
-// The plain (RESAMPLE == 0) path (DSB_GN_APPLY_V2=0 selects the older loop inside gn_apply_kernel<0> for A/B): the
-// normalisation is folded to one FMA per element, y = x * a + b' with b' = b - mean * a (16 instead of 24 live coefficient registers), and
-// four pixels are processed per iteration so that eight 16-byte loads are in flight per thread (the two-pixel loop keeps ~49 KB per SM in
-// flight, about the minimum HBM needs).
+// Resample 0: the normalisation is folded to one FMA per element, y = x * a + b' with b' = b - mean * a (16 instead of 24 live
+// coefficient registers), and four pixels are processed per iteration so that eight 16-byte loads are in flight per thread (two pixels
+// keep ~49 KB per SM in flight, about the minimum HBM needs).
 template <int NP>
 __device__ __forceinline__ void gn_v2_pixels(const ds_gn_apply_desc& d, const float* base, int pitch, long long n, int npix, int C, int c,
                                              long long plane, int po, int rows, bool norm, const float* a, const float* b, __half* oact,
@@ -370,9 +287,9 @@ __device__ __forceinline__ void gn_v2_pixels(const ds_gn_apply_desc& d, const fl
                 }
                 y[j] = u;
             }
-            gn_store_planes(oact, plane, o, y, d.nplanes, d.fmt);
+            store_operand<8>(oact, plane, o, y, d.nplanes, d.fmt);
         }
-        if (oraw) gn_store_planes(oraw, plane, o, e, d.nplanes, d.fmt);
+        if (oraw) store_operand<8>(oraw, plane, o, e, d.nplanes, d.fmt);
         if (d.out_raw_f32) {
             *reinterpret_cast<float4*>(d.out_raw_f32 + o) = v[k][0];
             *reinterpret_cast<float4*>(d.out_raw_f32 + o + 4) = v[k][1];
@@ -397,25 +314,14 @@ __global__ void __launch_bounds__(512) gn_apply_v2_kernel(ds_gn_apply_desc d, in
         for (int j = 0; j < 8; ++j) {
             const int g = (c + j) / cpg;
             if (g != g_prev) {
-                const double s = d.sums[((long long)n * d.groups + g) * 2 + 0];
-                const double q = d.sums[((long long)n * d.groups + g) * 2 + 1];
-                const double mu = s / cnt;
-                double var = q / cnt - mu * mu;
-                if (var < 0.0) var = 0.0;
-                rstd = (float)(1.0 / sqrt(var + (double)d.eps));
-                mu_f = (float)mu;
+                const float2 st = gn_group_stats(d, n, g, cnt);
+                mu_f = st.x;
+                rstd = st.y;
                 g_prev = g;
             }
-            float aa = rstd * __ldg(d.gamma + c + j);
-            float bb = __ldg(d.beta + c + j);
-            if (d.ada) {
-                const float sc = d.ada[(long long)n * d.ada_stride + c + j] + 1.0f;
-                const float sh = d.ada[(long long)n * d.ada_stride + C + c + j];
-                aa *= sc;
-                bb = bb * sc + sh;
-            }
-            a[j] = aa;
-            b[j] = fmaf(-mu_f, aa, bb);
+            float bb;
+            gn_channel_coef(d, n, C, c, j, rstd, a[j], bb);
+            b[j] = fmaf(-mu_f, a[j], bb);
         }
     }
     const int npix = d.H * d.W;
@@ -545,12 +451,7 @@ __global__ void __launch_bounds__(256) softmax_reg_kernel(ds_softmax_desc d) {
         const int j = (tid + k * nthr) * 4;
         if (j < d.L) {
             const float e[4] = {v[k].x * inv, v[k].y * inv, v[k].z * inv, v[k].w * inv};
-            __align__(8) __half hi[4];
-            __align__(8) __half lo[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) split_h16(e[q], hi[q], lo[q]);
-            *reinterpret_cast<uint2*>(P + row * d.L + j) = *reinterpret_cast<const uint2*>(hi);
-            if (d.nplanes > 1) *reinterpret_cast<uint2*>(P + plane + row * d.L + j) = *reinterpret_cast<const uint2*>(lo);
+            store_planes<4>(P, plane, row * d.L + j, e, d.nplanes);
         }
     }
 }
@@ -584,12 +485,7 @@ __global__ void softmax_kernel(ds_softmax_desc d) {
         for (int j = lane * 4; j < d.L; j += 128) {
             const float4 v = *reinterpret_cast<const float4*>(s + j);
             const float e[4] = {expf(v.x - m) * inv, expf(v.y - m) * inv, expf(v.z - m) * inv, expf(v.w - m) * inv};
-            __align__(8) __half hi[4];
-            __align__(8) __half lo[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) split_h16(e[k], hi[k], lo[k]);
-            *reinterpret_cast<uint2*>(P + row * pout + j) = *reinterpret_cast<const uint2*>(hi);
-            if (d.nplanes > 1) *reinterpret_cast<uint2*>(P + plane + row * pout + j) = *reinterpret_cast<const uint2*>(lo);
+            store_planes<4>(P, plane, row * pout + j, e, d.nplanes);
         }
         return;
     }
@@ -693,19 +589,13 @@ __global__ void prep_input_kernel(ds_prep_input_desc d) {
     const int xb = d.x_batch > 0 ? d.x_batch : d.B;
     const int nx = n % xb;
     const float cin = d.coef[nx * d.coef_stride + 2];
-    __align__(16) __half hi[8];
-    __align__(16) __half lo[8];
+    float v[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         const int c = c8 * 8 + j;
-        float v = 0.f;
-        if (c < d.C) v = cin * d.x[((long long)nx * d.C + c) * d.HW + hw];
-        split_h16(v, hi[j], lo[j]);
+        v[j] = c < d.C ? cin * d.x[((long long)nx * d.C + c) * d.HW + hw] : 0.f;
     }
-    __half* o = reinterpret_cast<__half*>(d.out);
-    const long long off = px * 64 + c8 * 8;
-    *reinterpret_cast<uint4*>(o + off) = *reinterpret_cast<const uint4*>(hi);
-    if (d.nplanes > 1) *reinterpret_cast<uint4*>(o + (long long)d.B * d.HW * 64 + off) = *reinterpret_cast<const uint4*>(lo);
+    store_planes<8>(reinterpret_cast<__half*>(d.out), (long long)d.B * d.HW * 64, px * 64 + c8 * 8, v, d.nplanes);
 }
 
 // Vector-quantized input: one thread per pixel holds v = c_in * x (channels zero-padded to CP) and streams the codebook through shared
@@ -762,19 +652,19 @@ __global__ void __launch_bounds__(256) vq_prep_input_kernel(ds_prep_input_desc d
     const long long plane = total * 64;
 #pragma unroll
     for (int c8 = 0; c8 < 8; ++c8) {
-        __align__(16) __half hi[8];
-        __align__(16) __half lo[8];
+        float e[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int c = c8 * 8 + j;
-            split_h16(c < d.C ? d.codebook[(long long)bi * d.C + c] : 0.f, hi[j], lo[j]);
+            e[j] = c < d.C ? d.codebook[(long long)bi * d.C + c] : 0.f;
         }
-        *reinterpret_cast<uint4*>(o + px * 64 + c8 * 8) = *reinterpret_cast<const uint4*>(hi);
-        if (d.nplanes > 1) *reinterpret_cast<uint4*>(o + plane + px * 64 + c8 * 8) = *reinterpret_cast<const uint4*>(lo);
+        store_planes<8>(o, plane, px * 64 + c8 * 8, e, d.nplanes);
     }
 }
 
-// one warp per token row; the row lives in registers (C <= 2048), two-pass mean / variance like torch's layer_norm
+// one warp per token row; the row lives in registers (C <= 2048), two-pass mean / variance like torch's layer_norm.
+// FMT (ds_layernorm_desc.fmt): 0 fp16 planes, 1 f8 image (operand.cuh), 2 fp32 [rows][C] (the last LayerNorm of the CLIP text encoder).
+template <int FMT>
 __global__ void layernorm_kernel(ds_layernorm_desc d) {
     const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= d.rows) return;
@@ -807,8 +697,6 @@ __global__ void layernorm_kernel(ds_layernorm_desc d) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
     const float rstd = rsqrtf(sq / (float)d.C + d.eps);
-    __half* out = reinterpret_cast<__half*>(d.out);
-    const long long plane = d.rows * d.C;
 #pragma unroll
     for (int k = 0; k < MAXV; ++k) {
         const int j = lane + 32 * k;
@@ -817,34 +705,10 @@ __global__ void layernorm_kernel(ds_layernorm_desc d) {
             const float4 b = *reinterpret_cast<const float4*>(d.beta + 4 * j);
             const float y[4] = {(v[k].x - mean) * rstd * g.x + b.x, (v[k].y - mean) * rstd * g.y + b.y,
                                 (v[k].z - mean) * rstd * g.z + b.z, (v[k].w - mean) * rstd * g.w + b.w};
-            if (d.fmt == 2) {                    // fp32 result (the last LayerNorm of the CLIP text encoder)
-                *reinterpret_cast<float4*>(reinterpret_cast<float*>(d.out) + row * d.C + 4 * j) = make_float4(y[0], y[1], y[2], y[3]);
-                continue;
-            }
-            __align__(8) __half hi[4];
-            __align__(8) __half lo[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) split_h16(y[q], hi[q], lo[q]);
-            *reinterpret_cast<uint2*>(out + row * d.C + 4 * j) = *reinterpret_cast<const uint2*>(hi);
-            if (d.nplanes > 1) *reinterpret_cast<uint2*>(out + plane + row * d.C + 4 * j) = *reinterpret_cast<const uint2*>(lo);
+            if (FMT == 2) *reinterpret_cast<float4*>(reinterpret_cast<float*>(d.out) + row * d.C + 4 * j) = make_float4(y[0], y[1], y[2], y[3]);
+            else store_operand<4>(reinterpret_cast<__half*>(d.out), d.rows * d.C, row * d.C + 4 * j, y, d.nplanes, FMT);
         }
     }
-}
-
-// quick-GELU (ds_geglu_desc.mode == 1): out = x * sigmoid(1.702 x) on fp32 [rows][I] -> fp16 hi/lo planes (CLIP MLP activation)
-__global__ void quick_gelu_kernel(ds_geglu_desc d) {
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;       // one thread per 4 values
-    const long long total = d.rows * (d.I / 4);
-    if (idx >= total) return;
-    const float4 a = *reinterpret_cast<const float4*>(d.src + idx * 4);
-    const float av[4] = {a.x, a.y, a.z, a.w};
-    __align__(8) __half hi[4];
-    __align__(8) __half lo[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) split_h16(av[q] / (1.0f + expf(-1.702f * av[q])), hi[q], lo[q]);
-    __half* out = reinterpret_cast<__half*>(d.out);
-    *reinterpret_cast<uint2*>(out + idx * 4) = *reinterpret_cast<const uint2*>(hi);
-    if (d.nplanes > 1) *reinterpret_cast<uint2*>(out + d.rows * d.I + idx * 4) = *reinterpret_cast<const uint2*>(lo);
 }
 
 // token + position embedding (ds_embed_desc): one thread per 4 channels of one row
@@ -861,105 +725,30 @@ __global__ void embed_kernel(ds_embed_desc d) {
     *reinterpret_cast<float4*>(d.out + row * d.C + j) = make_float4(t.x + p.x, t.y + p.y, t.z + p.z, t.w + p.w);
 }
 
-__global__ void geglu_kernel(ds_geglu_desc d) {
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;       // one thread per 4 outputs
-    const int i4 = d.I / 4;
-    const long long total = d.rows * i4;
-    if (idx >= total) return;
-    const long long row = idx / i4;
-    const int j = (int)(idx - row * i4) * 4;
-    const float4 a = *reinterpret_cast<const float4*>(d.src + row * 2 * d.I + j);
-    const float4 g = *reinterpret_cast<const float4*>(d.src + row * 2 * d.I + d.I + j);
-    const float av[4] = {a.x, a.y, a.z, a.w}, gv[4] = {g.x, g.y, g.z, g.w};
-    __align__(8) __half hi[4];
-    __align__(8) __half lo[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        const float gelu = 0.5f * gv[q] * (1.0f + erff(gv[q] * 0.70710678118654752f));
-        split_h16(av[q] * gelu, hi[q], lo[q]);
-    }
-    __half* out = reinterpret_cast<__half*>(d.out);
-    *reinterpret_cast<uint2*>(out + row * d.I + j) = *reinterpret_cast<const uint2*>(hi);
-    if (d.nplanes > 1) *reinterpret_cast<uint2*>(out + d.rows * d.I + row * d.I + j) = *reinterpret_cast<const uint2*>(lo);
-}
-
-// ---- f8 operand image (csrc/ops.h) of four consecutive values: fp16 (v * 2^A16) | e4m3 ((v - hi) * 2^LO8) | e4m3 (hi * 2^HI8) --------------
-// `plane` = elements per plane; o = element offset.  Same arithmetic as gn_store_f8 (which handles eight values).
-__device__ __forceinline__ void store4_f8(__half* base, long long plane, long long o, const float* v) {
-    __align__(8) uint32_t hi[2];
-    __align__(4) unsigned short lo8[2];
-    __align__(4) unsigned short hi8[2];
-#pragma unroll
-    for (int j = 0; j < 2; ++j) f8_image_pair(v[2 * j], v[2 * j + 1], hi[j], lo8[j], hi8[j]);
-    *reinterpret_cast<uint2*>(base + o) = *reinterpret_cast<const uint2*>(hi);
-    unsigned char* b8 = reinterpret_cast<unsigned char*>(base + plane);
-    *reinterpret_cast<unsigned int*>(b8 + o) = *reinterpret_cast<const unsigned int*>(lo8);
-    *reinterpret_cast<unsigned int*>(b8 + plane + o) = *reinterpret_cast<const unsigned int*>(hi8);
-}
-
-// LayerNorm / GEGLU writing the f8 operand image (fmt == 1; opt-in, feeds an f8 GEMM).  Separate kernels so that the default ones above
-// stay byte-identical; the arithmetic before the store is the same.
-__global__ void layernorm_f8_kernel(ds_layernorm_desc d) {
-    const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (row >= d.rows) return;
-    const int lane = threadIdx.x & 31;
-    const float* x = d.src + row * d.C;
-    constexpr int MAXV = 16;
-    float4 v[MAXV];
-    const int nv = d.C / 4;
-    float sum = 0.f;
-#pragma unroll
-    for (int k = 0; k < MAXV; ++k) {
-        const int j = lane + 32 * k;
-        if (j < nv) {
-            v[k] = *reinterpret_cast<const float4*>(x + 4 * j);
-            sum += v[k].x + v[k].y + v[k].z + v[k].w;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float mean = sum / (float)d.C;
-    float sq = 0.f;
-#pragma unroll
-    for (int k = 0; k < MAXV; ++k) {
-        const int j = lane + 32 * k;
-        if (j < nv) {
-            const float a = v[k].x - mean, b = v[k].y - mean, c = v[k].z - mean, e = v[k].w - mean;
-            sq += a * a + b * b + c * c + e * e;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-    const float rstd = rsqrtf(sq / (float)d.C + d.eps);
-    __half* out = reinterpret_cast<__half*>(d.out);
-    const long long plane = d.rows * d.C;
-#pragma unroll
-    for (int k = 0; k < MAXV; ++k) {
-        const int j = lane + 32 * k;
-        if (j < nv) {
-            const float4 g = *reinterpret_cast<const float4*>(d.gamma + 4 * j);
-            const float4 b = *reinterpret_cast<const float4*>(d.beta + 4 * j);
-            const float y[4] = {(v[k].x - mean) * rstd * g.x + b.x, (v[k].y - mean) * rstd * g.y + b.y,
-                                (v[k].z - mean) * rstd * g.z + b.z, (v[k].w - mean) * rstd * g.w + b.w};
-            store4_f8(out, plane, row * d.C + 4 * j, y);
-        }
-    }
-}
-
-__global__ void geglu_f8_kernel(ds_geglu_desc d) {
+// Gated activations (ds_geglu_desc), one thread per 4 outputs of [rows][I], written in format FMT (operand.cuh):
+//   MODE 0, GEGLU: out = x[:, :I] * gelu(x[:, I:]) on fp32 [rows][2I], exact erf GELU.
+//   MODE 1, quick-GELU: out = x * sigmoid(1.702 x) on fp32 [rows][I] (CLIP MLP activation).
+template <int MODE, int FMT>
+__global__ void gate_kernel(ds_geglu_desc d) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int i4 = d.I / 4;
-    const long long total = d.rows * i4;
-    if (idx >= total) return;
-    const long long row = idx / i4;
-    const int j = (int)(idx - row * i4) * 4;
-    const float4 a = *reinterpret_cast<const float4*>(d.src + row * 2 * d.I + j);
-    const float4 g = *reinterpret_cast<const float4*>(d.src + row * 2 * d.I + d.I + j);
-    const float av[4] = {a.x, a.y, a.z, a.w}, gv[4] = {g.x, g.y, g.z, g.w};
+    if (idx >= d.rows * i4) return;
     float y[4];
+    if (MODE == 0) {
+        const long long row = idx / i4;
+        const int j = (int)(idx - row * i4) * 4;
+        const float4 a = *reinterpret_cast<const float4*>(d.src + row * 2 * d.I + j);
+        const float4 g = *reinterpret_cast<const float4*>(d.src + row * 2 * d.I + d.I + j);
+        const float av[4] = {a.x, a.y, a.z, a.w}, gv[4] = {g.x, g.y, g.z, g.w};
 #pragma unroll
-    for (int q = 0; q < 4; ++q) y[q] = av[q] * (0.5f * gv[q] * (1.0f + erff(gv[q] * 0.70710678118654752f)));
-    store4_f8(reinterpret_cast<__half*>(d.out), d.rows * d.I, row * d.I + j, y);
+        for (int q = 0; q < 4; ++q) y[q] = av[q] * (0.5f * gv[q] * (1.0f + erff(gv[q] * 0.70710678118654752f)));
+    } else {
+        const float4 a = *reinterpret_cast<const float4*>(d.src + idx * 4);
+        const float av[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) y[q] = av[q] / (1.0f + expf(-1.702f * av[q]));
+    }
+    store_operand<4>(reinterpret_cast<__half*>(d.out), d.rows * d.I, idx * 4, y, d.nplanes, FMT);
 }
 
 __global__ void chanmean_kernel(ds_chanmean_desc d) {
@@ -1065,15 +854,10 @@ extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream
         gn_apply_v3_kernel<<<(unsigned)g3, threads, 0, stream>>>(*d, nc8, rows, ups, total_units);
         return ok();
     }
-    static const int use_v2 = [] { const char* e = getenv("DSB_GN_APPLY_V2"); return e ? atoi(e) : 1; }();
-    if (use_v2 && d->resample == 0) {
-        gn_apply_v2_kernel<<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
-        return ok();
-    }
     if (d->resample == 1) gn_apply_kernel<1><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
     else if (d->resample == 3) gn_apply_kernel<3><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
     else if (d->resample == 2) gn_apply_kernel<2><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
-    else gn_apply_kernel<0><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
+    else gn_apply_v2_kernel<<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
     return ok();
 }
 
@@ -1087,29 +871,30 @@ extern "C" int ds_embed_launch(const ds_embed_desc* d, cudaStream_t stream) {
 extern "C" int ds_layernorm_launch(const ds_layernorm_desc* d, cudaStream_t stream) {
     if (d->C % 4 || d->C > 2048) return -2;
     const int wpb = 8;
+    const unsigned blocks = (unsigned)((d->rows + wpb - 1) / wpb);
     if (d->fmt == 1) {
         if (d->nplanes != 2) return -2;
-        layernorm_f8_kernel<<<(unsigned)((d->rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(*d);
-        return ok();
+        layernorm_kernel<1><<<blocks, wpb * 32, 0, stream>>>(*d);
+    } else if (d->fmt == 2) {
+        layernorm_kernel<2><<<blocks, wpb * 32, 0, stream>>>(*d);
+    } else {
+        layernorm_kernel<0><<<blocks, wpb * 32, 0, stream>>>(*d);
     }
-    layernorm_kernel<<<(unsigned)((d->rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(*d);
     return ok();
 }
 
 extern "C" int ds_geglu_launch(const ds_geglu_desc* d, cudaStream_t stream) {
     if (d->I % 4) return -2;
-    const long long total = d->rows * (d->I / 4);
+    const unsigned blocks = (unsigned)((d->rows * (d->I / 4) + 255) / 256);
     if (d->mode == 1) {
         if (d->fmt != 0) return -2;
-        quick_gelu_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(*d);
-        return ok();
-    }
-    if (d->fmt == 1) {
+        gate_kernel<1, 0><<<blocks, 256, 0, stream>>>(*d);
+    } else if (d->fmt == 1) {
         if (d->nplanes != 2) return -2;
-        geglu_f8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(*d);
-        return ok();
+        gate_kernel<0, 1><<<blocks, 256, 0, stream>>>(*d);
+    } else {
+        gate_kernel<0, 0><<<blocks, 256, 0, stream>>>(*d);
     }
-    geglu_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(*d);
     return ok();
 }
 
