@@ -56,7 +56,7 @@ class SoftmaxDesc(C.Structure):
 
 class PosembDesc(C.Structure):
     _fields_ = [('sigma', P), ('nsig', I32), ('num_channels', I32), ('endpoint', I32), ('swap_sincos', I32),
-                ('sigma_data', F32), ('mode', I32), ('coef', P), ('emb', P)]
+                ('sigma_data', F32), ('mode', I32), ('coef', P), ('emb', P), ('noise_scale', F32), ('pad0', I32)]
 
 
 class LinearDesc(C.Structure):

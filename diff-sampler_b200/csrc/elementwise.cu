@@ -532,12 +532,14 @@ __global__ void posemb_kernel(ds_posemb_desc d) {
         d.coef[n * 4 + 2] = 1.0f / sqrtf(s2);
         d.coef[n * 4 + 3] = c_noise;
     }
+    // CMPrecond feeds 1000 * c_noise to its U-Net's timestep_embedding (networks_edm.py:539-540)
+    const float t_emb = d.noise_scale != 0.0f ? d.noise_scale * c_noise : c_noise;
     const int half = d.num_channels / 2;
     for (int i = threadIdx.x; i < half; i += blockDim.x) {
         // freqs = (1/10000) ** (i / (half - endpoint))   (networks_edm.py:193-195)
         const float fr = (float)i / (float)(half - (d.endpoint ? 1 : 0));
         const float freq = powf(1.0f / 10000.0f, fr);
-        const float a = c_noise * freq;
+        const float a = t_emb * freq;
         const float cs = cosf(a), sn = sinf(a);
         // reference layout is [cos | sin]; SongUNet then swaps the halves to [sin | cos]
         if (d.swap_sincos) { d.emb[n * d.num_channels + i] = sn; d.emb[n * d.num_channels + half + i] = cs; }

@@ -209,6 +209,8 @@ typedef struct ds_posemb_desc {
                             //    `sigma` holds the timesteps, emb = [cos(t f_i) | sin(t f_i)], f_i = exp(-ln(1e4) i / half); coef untouched
     float* coef;            // [nsig][4] = (c_skip, c_out, c_in, c_noise)
     float* emb;             // [nsig][num_channels]
+    float noise_scale;      // mode 0: the embedding argument is noise_scale * c_noise (Consistency Models: 1000); 0 means 1
+    int32_t pad0;
 } ds_posemb_desc;
 
 // Small dense layer on CUDA cores (embedding MLP and all per-block affines in one launch):

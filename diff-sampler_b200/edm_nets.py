@@ -202,6 +202,7 @@ class NetSpec:
     sigma_max: float = 80.0
     prefix: str = 'model.'
     bottleneck_block: Optional[str] = None
+    noise_scale: float = 1.0         # the embedding reads noise_scale * ln(sigma) / 4 (1: EDM, 1000: Consistency Models' CMPrecond)
 
 
 def spec_from_params(params, img_resolution, img_channels, label_dim, prefix='model.'):

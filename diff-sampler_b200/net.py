@@ -35,7 +35,7 @@ def default_cuda_graph():
 
 class B200Net:
     def __init__(self, params, img_resolution, img_channels, label_dim=0, sigma_min=0.002, sigma_max=80.0, sigma_data=0.5,
-                 precision=None, device='cuda', fuse_stats=True, flash_attn=True, f8_min_channels=None, cuda_graph=None):
+                 precision=None, device='cuda', fuse_stats=True, flash_attn=True, f8_min_channels=None, cuda_graph=None, spec=None):
         self.device = torch.device(device)
         precision = precision or default_precision()
         if self.device.type != 'cuda':
@@ -53,7 +53,8 @@ class B200Net:
         self.fuse_stats = bool(fuse_stats)
         self.flash_attn = bool(flash_attn)
         self.cuda_graph = default_cuda_graph() if cuda_graph is None else bool(cuda_graph)
-        self.spec = edm_nets.spec_from_params(params, img_resolution, img_channels, label_dim)
+        # spec: the block structure when the parameter names cannot carry it (Consistency-Models nets, cm_net.py)
+        self.spec = spec if spec is not None else edm_nets.spec_from_params(params, img_resolution, img_channels, label_dim)
         self.spec.sigma_data = sigma_data
         self.wb, self.winfo = planner.pack_weights(self.spec, params, f8=self.f8, f8_min_channels=self.f8_min_channels)
         blob = self.wb.bytes()
@@ -90,6 +91,31 @@ class B200Net:
         net = cls(params, meta['img_resolution'], meta['img_channels'], meta['label_dim'], **kw)
         net.checkpoint_meta = meta
         return net
+
+    @classmethod
+    def from_cm(cls, net, setting=None, **kw):
+        """Compile a reference CMPrecond module (networks_edm.py:504-549) around a Consistency-Models UNetModel built with `setting`
+        (default: cm_model_loader.lsun_setting(), the lsun_bedroom / lsun_cat nets)."""
+        from . import cm_net
+        if getattr(net, 'label_dim', 0):
+            raise ValueError('label_dim: class-conditional CM nets are not lowered')
+        spec, params = cm_net.convert(net.state_dict(), setting, prefix='model.')
+        if int(net.img_resolution) != spec.img_resolution:
+            raise ValueError(f'img_resolution={net.img_resolution} does not match the settings ({spec.img_resolution})')
+        return cls(params, spec.img_resolution, spec.img_channels, 0, sigma_min=float(net.sigma_min), sigma_max=float(net.sigma_max),
+                   sigma_data=float(net.sigma_data), spec=spec, **kw)
+
+    @classmethod
+    def from_cm_checkpoint(cls, f, setting=None, **kw):
+        """Load a released Consistency-Models checkpoint (edm_bedroom256_ema.pt, edm_cat256_ema.pt: a UNetModel state dict) from a path
+        or file object, with torch.load(weights_only=True), and wrap it as sample.py does (CMPrecond defaults: sigma in [0.002, 80],
+        sigma_data 0.5)."""
+        from . import cm_net
+        sd = torch.load(f, map_location='cpu', weights_only=True)
+        spec, params = cm_net.convert(sd, setting)
+        for k, v in (('sigma_min', 0.002), ('sigma_max', 80.0), ('sigma_data', 0.5)):
+            kw.setdefault(k, v)
+        return cls(params, spec.img_resolution, spec.img_channels, 0, spec=spec, **kw)
 
     # ---- plan cache -------------------------------------------------------------------------------------------------
     @property

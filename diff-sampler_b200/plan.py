@@ -380,7 +380,8 @@ def compile_plan(spec, wb, winfo, B, nsig, nlab, npass=3, fuse_stats=True, flash
     pb.stats(2 * len(spec.enc + spec.dec) + sum(1 for b in spec.enc + spec.dec if b.heads) + 1)
     emit(lambda R: S.PosembDesc(sigma=io(S.DS_IO_SIGMA), nsig=nsig, num_channels=spec.noise_channels,
                                 endpoint=1 if spec.kind == 'song' else 0, swap_sincos=1 if spec.kind == 'song' else 0,
-                                sigma_data=spec.sigma_data, coef=R('coef'), emb=R('emb0')))
+                                sigma_data=spec.sigma_data, coef=R('coef'), emb=R('emb0'),
+                                noise_scale=0.0 if spec.noise_scale == 1 else spec.noise_scale))     # 0: the kernel's default of 1
     nc, ec = spec.noise_channels, spec.emb_channels
     if spec.kind == 'song':
         src, src_rows = 'emb0', nsig
