@@ -10,6 +10,13 @@ __device__ __forceinline__ void st4(float* p, long long i4, float4 v) { __stcs(r
 
 __device__ __forceinline__ int b_of(long long i4, long long n4_per_sample) { return (int)(i4 / n4_per_sample); }
 
+// (v * 127.5 + 128).clip(0, 255).to(uint8) as sample.py:311 evaluates it in fp32: the product and the sum are rounded separately.
+// A contracted FFMA rounds once and truncates to one less for inputs within an ulp of a boundary (N - 128) / 127.5;
+// __fmul_rn / __fadd_rn are never contracted.  NaN maps to 0: fmaxf returns the non-NaN operand.
+__device__ __forceinline__ unsigned char image_u8(float v) {
+    return (unsigned char)fminf(fmaxf(__fadd_rn(__fmul_rn(v, 127.5f), 128.0f), 0.0f), 255.0f);
+}
+
 template <int NH, int MODE>
 __global__ void __launch_bounds__(256) update_kernel(ds_update_desc d, long long n4_total, long long n4_per_sample) {
     const long long stride = (long long)gridDim.x * blockDim.x;
@@ -55,7 +62,7 @@ __global__ void __launch_bounds__(256) update_kernel(ds_update_desc d, long long
             unsigned char* dst = d.out_u8 + ((long long)b_of(i, n4_per_sample) * d.u8_HW + p) * d.u8_C + c;
             const float v[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
-            for (int k = 0; k < 4; ++k) dst[(long long)k * d.u8_C] = (unsigned char)fminf(fmaxf(v[k] * 127.5f + 128.0f, 0.0f), 255.0f);
+            for (int k = 0; k < 4; ++k) dst[(long long)k * d.u8_C] = image_u8(v[k]);
         }
     }
 }
@@ -273,11 +280,7 @@ __global__ void to_uint8_nhwc_kernel(const float* x, unsigned char* out, int B, 
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;       // one thread per (n, pixel)
     if (idx >= (long long)B * HW) return;
     const int n = (int)(idx / HW), p = (int)(idx - (long long)n * HW);
-    for (int c = 0; c < Cc; ++c) {
-        float v = x[((long long)n * Cc + c) * HW + p] * 127.5f + 128.0f;
-        v = fminf(fmaxf(v, 0.0f), 255.0f);
-        out[idx * Cc + c] = (unsigned char)v;                                      // truncation, as torch's float -> uint8 cast
-    }
+    for (int c = 0; c < Cc; ++c) out[idx * Cc + c] = image_u8(x[((long long)n * Cc + c) * HW + p]);
 }
 
 }  // namespace dsb
