@@ -77,27 +77,32 @@ struct SmemCtl {
 // Sum NV per-lane values over the 32 lanes of a warp with NV-ish shuffles instead of 5*NV: at every butterfly level each lane
 // keeps one half of its values and hands the other half to its partner, so the value count halves while the lane span doubles.
 // On return v[0] of lane L is the full sum of value index (L >> (5 - log2 NV)) (NV = 16: L >> 1; NV = 8: L >> 2).
+// The levels recurse on a template count: with a runtime count (n >>= 1) the level loop stays rolled, v[i + n] becomes a dynamic
+// index and the whole array moves to the stack.
+template <int N>
+__device__ __forceinline__ void warp_sum_levels(float* v, int lane, int off) {
+    if constexpr (N >= 1) {
+        const bool up = (lane & off) != 0;
+#pragma unroll
+        for (int i = 0; i < N; ++i) {
+            const float send = up ? v[i] : v[i + N];
+            const float keep = up ? v[i + N] : v[i];
+            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+        }
+        warp_sum_levels<N / 2>(v, lane, off >> 1);
+    } else {
+        for (; off >= 1; off >>= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], off);
+    }
+}
 template <int NV>
 __device__ __forceinline__ void warp_sum_multi(float (&v)[NV], int lane) {
     static_assert(NV == 32 || NV == 16 || NV == 8, "NV");
-    int off = 16;
-#pragma unroll
-    for (int n = NV / 2; n >= 1; n >>= 1) {
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < n; ++i) {
-            const float send = up ? v[i] : v[i + n];
-            const float keep = up ? v[i + n] : v[i];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-        off >>= 1;
-    }
-    for (; off >= 1; off >>= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], off);
+    warp_sum_levels<NV / 2>(v, lane, 16);
 }
 
 template <int W>
 __device__ __forceinline__ void epilogue_chunk(const GemmKernelParams& p, const float* v, long long grow_in_z, int col0, bool row_ok,
-                                               int zb, int zh, const float4* res_pref, bool res_in_regs) {
+                                               int zb, int zh) {
     // v[W]: accumulators of this thread's row, columns col0 .. col0+W-1 (col0 is the global column)
     const bool warp_rows_ok = __all_sync(0xffffffffu, row_ok);      // every lane has a valid row: the paired stores below may shuffle
     if (!row_ok) return;                                   // warp-uniform whenever statistics are fused (m_valid % 32 == 0)
@@ -139,25 +144,17 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKernelParams& p, const 
         }
     }
     if (p.residual) {
-        if (res_in_regs) {
+        const float* rs = p.residual + grow_in_z * p.ldr + col0;
+        if (full) {
 #pragma unroll
             for (int j = 0; j < W; j += 4) {
-                const float4 t = res_pref[j >> 2];
+                const float4 t = *reinterpret_cast<const float4*>(rs + j);
                 r[j] += t.x; r[j + 1] += t.y; r[j + 2] += t.z; r[j + 3] += t.w;
             }
         } else {
-            const float* rs = p.residual + grow_in_z * p.ldr + col0;
-            if (full) {
 #pragma unroll
-                for (int j = 0; j < W; j += 4) {
-                    const float4 t = *reinterpret_cast<const float4*>(rs + j);
-                    r[j] += t.x; r[j + 1] += t.y; r[j + 2] += t.z; r[j + 3] += t.w;
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < W; ++j)
-                    if (col0 + j < p.n_valid) r[j] += rs[j];
-            }
+            for (int j = 0; j < W; ++j)
+                if (col0 + j < p.n_valid) r[j] += rs[j];
         }
     }
 #pragma unroll
@@ -371,37 +368,53 @@ __device__ __forceinline__ void producer_tile(const GemmKernelParams& p, uint8_t
 }
 
 // ------------------------------------------------------------------------------------------ consumer: the K loop of one tile
-// One consumer warpgroup, 64 rows: per ring stage one wgmma group; the stage before it is released once only the newest group is
-// still in flight.
+// One consumer warpgroup, 64 rows.  Walks the ring in the producer's order; every stage is one wgmma group, issued and committed in
+// one straight block (fence, its MMAs, commit).  ptxas then marks only the group's last MMA as the commit point, so the wait for
+// "one group in flight" really leaves this stage's MMAs running and retires the previous stage, which is released at once.  Keep
+// the commit in that block: after a branch merge ptxas carries it on an empty MMA of its own, the wait drains every real MMA, and
+// the consumers hold one retired stage the producer could already refill (tests/test_gemm_sass.py).
 template <int BN>
 __device__ __forceinline__ void mma_tile(const GemmKernelParams& p, uint8_t* smem, SmemCtl* ctl, RingPos& r, const int block_bytes,
-                                         const int n_iters, const int nkb8, const int wg, float (&acc)[BN / 2]) {
+                                         const int wg, float (&acc)[BN / 2]) {
     const bool leader = (threadIdx.x & 127) == 0;
     int prev = -1;
-    for (int it = 0; it < n_iters; ++it) {
+    uint32_t scale0 = 0u;                      // only the tile's first MMA overwrites the accumulators
+    auto stage = [&](auto f8, auto steps) {
+        constexpr bool F8 = decltype(f8)::value;
+        constexpr int NS = decltype(steps)::value;
         mbar_wait(&ctl->full[r.stage], r.phase);
         const uint32_t s0 = smem_u32(smem + r.stage * block_bytes);
         const uint64_t da = wgmma_desc_sw128(s0 + wg * 64 * 128);
         const uint64_t db = wgmma_desc_sw128(s0 + kATileBytes);
         wgmma_fence();
-        if (it < 2 * nkb8) {
-            // e4m3 blocks of a pass: taps x cpb8 main blocks (the last of each tap may be half empty), then the aux blocks
-            const int q8 = it < nkb8 ? it : it - nkb8;
-            const int ns = (q8 < p.nkb8_main && q8 % p.cpb8 == p.cpb8 - 1) ? p.f8_last_steps : 4;
 #pragma unroll
-            for (int k = 0; k < 4; ++k)        // 32 e4m3 = 32 bytes per MMA: the same +2 descriptor step (16-byte units) as 16 fp16
-                if (k < ns) wgmma_ss<BN, true>(acc, da + 2 * k, db + 2 * k, (it > 0 || k > 0) ? 1u : 0u);
-        } else {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) wgmma_ss<BN, false>(acc, da + 2 * k, db + 2 * k, (it > 0 || k > 0) ? 1u : 0u);
-        }
+        for (int k = 0; k < NS; ++k)           // 32 e4m3 = 32 bytes per MMA: the same +2 descriptor step (16-byte units) as 16 fp16
+            wgmma_ss<BN, F8>(acc, da + 2 * k, db + 2 * k, k > 0 ? 1u : scale0);
         wgmma_commit();
         wgmma_fence_regs(acc);
         wgmma_wait<1>();
         if (prev >= 0 && leader) mbar_arrive(&ctl->empty[prev]);
         prev = r.stage;
         if (++r.stage == p.num_stages) { r.stage = 0; r.phase ^= 1; }
+        scale0 = 1u;
+    };
+    using f8_t = std::true_type;
+    using f16_t = std::false_type;
+    using full_t = std::integral_constant<int, 4>;
+    using half_t = std::integral_constant<int, 2>;
+    if (p.f8) {
+        // e4m3 blocks of a pass: per tap cpb8 channel blocks (the last one half empty when f8_last_steps == 2), then the aux blocks
+        const int full8 = p.f8_last_steps == 2 ? p.cpb8 - 1 : p.cpb8;
+        for (int pass8 = 0; pass8 < 2; ++pass8) {
+            for (int tap = 0; tap < p.taps; ++tap) {
+                for (int cb = 0; cb < full8; ++cb) stage(f8_t{}, full_t{});
+                if (full8 < p.cpb8) stage(f8_t{}, half_t{});
+            }
+            for (int j = 0; j < p.nkb8_aux; ++j) stage(f8_t{}, full_t{});
+        }
     }
+    const int n16 = (p.f8 ? 1 : p.npass) * (p.nkb_main + p.nkb_aux);
+    for (int i = 0; i < n16; ++i) stage(f16_t{}, full_t{});
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     if (prev >= 0 && leader) mbar_arrive(&ctl->empty[prev]);
@@ -463,12 +476,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmKernelParams& p, float* 
             float v[32];
 #pragma unroll
             for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(v + j) = lds_f4(rkey ^ (4 * j));
-            if (col0 < p.n_valid) epilogue_chunk<32>(p, v, grow, col0, row_ok, tc.zb, tc.zh, nullptr, false);
+            if (col0 < p.n_valid) epilogue_chunk<32>(p, v, grow, col0, row_ok, tc.zb, tc.zh);
         } else if (width >= 16) {
             float v[16];
 #pragma unroll
             for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(v + j) = lds_f4(rkey ^ (4 * j));
-            if (col0 < p.n_valid) epilogue_chunk<16>(p, v, grow, col0, row_ok, tc.zb, tc.zh, nullptr, false);
+            if (col0 < p.n_valid) epilogue_chunk<16>(p, v, grow, col0, row_ok, tc.zb, tc.zh);
         }
         warpgroup_sync(1 + wg);
     }
@@ -485,10 +498,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
 
     const int warp = threadIdx.x >> 5;
     const int wg = threadIdx.x >> 7;
-    const int nkb_total = p.nkb_main + p.nkb_aux;
-    // f8 mode: 2 * nkb8 e4m3 blocks (A_lo8 x W_hi8, then A_hi8 x W_lo8; 128 channels each) followed by the nkb_total fp16 hi x hi blocks
-    const int nkb8 = p.f8 ? p.nkb8_main + p.nkb8_aux : 0;
-    const int n_iters = p.f8 ? 2 * nkb8 + nkb_total : p.npass * nkb_total;
     const int total_tiles = p.num_z * p.m_tiles * p.n_tiles;
 
     if (threadIdx.x == 0) {
@@ -545,7 +554,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const TileCoord tc = tile_coord(p, tile);
             float acc[BN / 2];
-            mma_tile<BN>(p, smem, ctl, ring, block_bytes, n_iters, nkb8, cw, acc);
+            mma_tile<BN>(p, smem, ctl, ring, block_bytes, cw, acc);
             epilogue_tile<BN>(p, my_stg, cw, tc, acc);
         }
     }
