@@ -772,7 +772,9 @@ using namespace dsb;
 
 extern "C" int ds_gn_stats_launch(const ds_gn_stats_desc* d, cudaStream_t stream) {
     const int C = d->C0 + d->C1;
-    if (C % 4 || d->groups > 64 || C % d->groups || (d->C0 % 4)) return -2;
+    if (C % 4 || d->groups <= 0 || d->groups > 64 || C % d->groups || (d->C0 % 4)) return -2;
+    // gn_stats_kernel splits a float4 column between at most two groups (gA / gB): groups of one channel would be summed into the wrong group
+    if (C / d->groups < 2) return -2;
     const int ncol4 = C / 4;
     int bx = ncol4 < 256 ? ncol4 : 256;
     // keep bx a divisor-friendly size; columns loop with stride bx anyway
@@ -819,6 +821,11 @@ extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream
     const int C = d->C0 + d->C1;
     if (C % 8 || (d->C0 % 8)) return -2;
     if (d->fmt != 0 && (d->fmt != 1 || d->resample == 3 || d->nplanes != 2)) return -2;   // the f8 layout reuses the two-plane footprint
+    // the coefficient table is read by the resample-0 kernel only; the resampling kernels normalise from the sums
+    if (d->coef && d->resample != 0) return -2;
+    if (d->out_act && !d->sums && !d->coef) return -2;                                      // a normalised output needs statistics
+    // 2x2 pooling and space-to-depth take whole 2x2 blocks: an odd row or column has no output pixel
+    if ((d->resample == 1 || d->resample == 3) && (d->H % 2 || d->W % 2)) return -2;
     const int nc8 = C / 8;
     if (nc8 > 512) return -2;
     int rows = 256 / nc8;

@@ -160,11 +160,15 @@ def _launcher_guard(op):
             return 'channels'
         if d.coef and d.resample == 0 and not d.sums and nc8 * max(1, 256 // nc8) > 256:
             return 'coef width'
-        if d.resample == 1 and (d.H % 2 or d.W % 2):
-            return 'pool'
+        if d.coef and d.resample != 0:
+            return 'coef resample'
+        if d.out_act and not d.sums and not d.coef:
+            return 'statistics'
+        if d.resample in (1, 3) and (d.H % 2 or d.W % 2):
+            return 'resample parity'
     elif t == S.DS_OP_GN_STATS:
         C = d.C0 + d.C1
-        if C % 4 or d.groups > 64 or C % d.groups or d.C0 % 4:
+        if C % 4 or d.groups <= 0 or d.groups > 64 or C % d.groups or d.C0 % 4 or C // d.groups < 2:
             return 'channels'
     elif t == S.DS_OP_GN_FINALIZE:
         C = d.C0 + d.C1
