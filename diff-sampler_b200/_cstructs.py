@@ -9,9 +9,14 @@ F32 = C.c_float
 
 DS_OP_GEMM, DS_OP_GN_STATS, DS_OP_GN_APPLY, DS_OP_SOFTMAX, DS_OP_POSEMB, DS_OP_LINEAR = 1, 2, 3, 4, 5, 6
 DS_OP_PREP_INPUT, DS_OP_CHANMEAN, DS_OP_MEMSET, DS_OP_LAYERNORM, DS_OP_GEGLU, DS_OP_GN_FINALIZE, DS_OP_ATTN, DS_OP_EMBED = 7, 8, 9, 10, 11, 12, 13, 14
+DS_OP_OPT_PREP, DS_OP_OPT_SOFTMAX, DS_OP_OPT_REDUCE, DS_OP_OPT_KNN = 15, 16, 17, 18
 DS_IO_X, DS_IO_D, DS_IO_SIGMA, DS_IO_LABELS, DS_IO_BOTTLENECK, DS_IO_CTX, DS_IO_COUNT = 0, 1, 2, 3, 4, 5, 6
 DS_M_X0, DS_M_EPS, DS_M_DIV, DS_M_NONE = 0, 1, 2, 3
 DS_F8_SH_A16, DS_F8_SH_LO8, DS_F8_SH_HI8 = 6, 13, 2      # csrc/ops.h: power-of-two operand scales of the f8 GEMM mode
+# csrc/ops.h: optimal-denoiser constants (band cap, P scale, band width in nats, rescoring threshold tau, u error per ||x|| ||y||)
+DS_OPT_CAP, DS_OPT_P_SHIFT, DS_OPT_BAND_NATS, DS_OPT_TAU, DS_OPT_EPS = 1024, 15, 40, 0.01, 2.0 ** -17
+DS_OPT_PLAIN, DS_OPT_RESCORED, DS_OPT_UNREFINED = 0, 1, 2
+DS_KNN_MAX, DS_KNN_CAND = 64, 256
 
 SPACE_ABS, SPACE_ARENA, SPACE_WEIGHTS, SPACE_IO = 0, 1, 2, 3
 
@@ -97,6 +102,24 @@ class EmbedDesc(C.Structure):
     _fields_ = [('ids', P), ('tok', P), ('pos', P), ('out', P), ('rows', I64), ('T', I32), ('C', I32), ('vocab', I32), ('pad0', I32)]
 
 
+class OptPrepDesc(C.Structure):
+    _fields_ = [('x', P), ('planes', P), ('xn2', P), ('B', I32), ('D', I32), ('pitch', I32), ('pad0', I32)]
+
+
+class OptSoftmaxDesc(C.Structure):
+    _fields_ = [('part', P), ('hy2', P), ('xn2', P), ('sigma', P), ('x', P), ('y', P), ('P', P), ('status', P), ('ldp', I64), ('ldP', I64),
+                ('B', I32), ('N', I32), ('D', I32), ('nslice', I32), ('nsig', I32), ('ymax', F32)]
+
+
+class OptReduceDesc(C.Structure):
+    _fields_ = [('part', P), ('out', P), ('rows', I64), ('cols', I32), ('ld', I32), ('nsplit', I32), ('scale', F32)]
+
+
+class OptKnnDesc(C.Structure):
+    _fields_ = [('part', P), ('hy2', P), ('xn2', P), ('x', P), ('y', P), ('dist', P), ('idx', P), ('ldp', I64),
+                ('B', I32), ('N', I32), ('D', I32), ('nslice', I32), ('k', I32), ('ymax', F32)]
+
+
 class MemsetDesc(C.Structure):
     _fields_ = [('ptr', P), ('bytes', I64)]
 
@@ -105,7 +128,8 @@ class _OpUnion(C.Union):
     _fields_ = [('gemm', GemmDesc), ('gn_stats', GnStatsDesc), ('gn_apply', GnApplyDesc), ('softmax', SoftmaxDesc),
                 ('posemb', PosembDesc), ('linear', LinearDesc), ('prep_input', PrepInputDesc), ('chanmean', ChanmeanDesc),
                 ('memset', MemsetDesc), ('layernorm', LayernormDesc), ('geglu', GegluDesc), ('gn_finalize', GnFinalizeDesc), ('attn', AttnDesc),
-                ('embed', EmbedDesc)]
+                ('embed', EmbedDesc), ('opt_prep', OptPrepDesc), ('opt_softmax', OptSoftmaxDesc), ('opt_reduce', OptReduceDesc),
+                ('opt_knn', OptKnnDesc)]
 
 
 class PlanOp(C.Structure):
@@ -116,15 +140,21 @@ SIZEOF_CHECKS = {
     0: PlanOp, DS_OP_GEMM: GemmDesc, DS_OP_GN_STATS: GnStatsDesc, DS_OP_GN_APPLY: GnApplyDesc, DS_OP_SOFTMAX: SoftmaxDesc,
     DS_OP_POSEMB: PosembDesc, DS_OP_LINEAR: LinearDesc, DS_OP_PREP_INPUT: PrepInputDesc, DS_OP_CHANMEAN: ChanmeanDesc,
     DS_OP_MEMSET: MemsetDesc, DS_OP_LAYERNORM: LayernormDesc, DS_OP_GEGLU: GegluDesc, DS_OP_GN_FINALIZE: GnFinalizeDesc, DS_OP_ATTN: AttnDesc,
-    DS_OP_EMBED: EmbedDesc,
+    DS_OP_EMBED: EmbedDesc, DS_OP_OPT_PREP: OptPrepDesc, DS_OP_OPT_SOFTMAX: OptSoftmaxDesc, DS_OP_OPT_REDUCE: OptReduceDesc,
+    DS_OP_OPT_KNN: OptKnnDesc,
 }
 
+# Union member of each op type of the network plans (plan.py, ldm_plan.py, vae_plan.py, clip_plan.py) ...
 UNION_FIELD = {
     DS_OP_GEMM: 'gemm', DS_OP_GN_STATS: 'gn_stats', DS_OP_GN_APPLY: 'gn_apply', DS_OP_SOFTMAX: 'softmax', DS_OP_POSEMB: 'posemb',
     DS_OP_LINEAR: 'linear', DS_OP_PREP_INPUT: 'prep_input', DS_OP_CHANMEAN: 'chanmean', DS_OP_MEMSET: 'memset',
     DS_OP_LAYERNORM: 'layernorm', DS_OP_GEGLU: 'geglu', DS_OP_GN_FINALIZE: 'gn_finalize', DS_OP_ATTN: 'attn', DS_OP_EMBED: 'embed',
 }
+# ... and of the ops only the optimal-denoiser plans (optimal.py) use around their two GEMMs.
+OPT_UNION_FIELD = {DS_OP_OPT_PREP: 'opt_prep', DS_OP_OPT_SOFTMAX: 'opt_softmax', DS_OP_OPT_REDUCE: 'opt_reduce', DS_OP_OPT_KNN: 'opt_knn'}
+ALL_UNION_FIELD = {**UNION_FIELD, **OPT_UNION_FIELD}
 OP_TYPE_OF = {GemmDesc: DS_OP_GEMM, GnStatsDesc: DS_OP_GN_STATS, GnApplyDesc: DS_OP_GN_APPLY, SoftmaxDesc: DS_OP_SOFTMAX,
               PosembDesc: DS_OP_POSEMB, LinearDesc: DS_OP_LINEAR, PrepInputDesc: DS_OP_PREP_INPUT, ChanmeanDesc: DS_OP_CHANMEAN,
               MemsetDesc: DS_OP_MEMSET, LayernormDesc: DS_OP_LAYERNORM, GegluDesc: DS_OP_GEGLU, GnFinalizeDesc: DS_OP_GN_FINALIZE, AttnDesc: DS_OP_ATTN,
-              EmbedDesc: DS_OP_EMBED}
+              EmbedDesc: DS_OP_EMBED, OptPrepDesc: DS_OP_OPT_PREP, OptSoftmaxDesc: DS_OP_OPT_SOFTMAX, OptReduceDesc: DS_OP_OPT_REDUCE,
+              OptKnnDesc: DS_OP_OPT_KNN}

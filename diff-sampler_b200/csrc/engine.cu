@@ -99,6 +99,10 @@ static void visit_ptrs(ds_plan_op& op, F f) {
         case DS_OP_GN_FINALIZE: { auto& d = op.u.gn_finalize; P(d.quads0); P(d.quads1); P(d.sums); P(d.gamma); P(d.beta); P(d.ada); P(d.coef); break; }
         case DS_OP_ATTN: { auto& d = op.u.attn; P(d.q); P(d.k); P(d.vt); P(d.out); break; }
         case DS_OP_EMBED: { auto& d = op.u.embed; P(d.ids); P(d.tok); P(d.pos); P(d.out); break; }
+        case DS_OP_OPT_PREP: { auto& d = op.u.opt_prep; P(d.x); P(d.planes); P(d.xn2); break; }
+        case DS_OP_OPT_SOFTMAX: { auto& d = op.u.opt_softmax; P(d.part); P(d.hy2); P(d.xn2); P(d.sigma); P(d.x); P(d.y); P(d.P); P(d.status); break; }
+        case DS_OP_OPT_REDUCE: { auto& d = op.u.opt_reduce; P(d.part); P(d.out); break; }
+        case DS_OP_OPT_KNN: { auto& d = op.u.opt_knn; P(d.part); P(d.hy2); P(d.xn2); P(d.x); P(d.y); P(d.dist); P(d.idx); break; }
         default: break;
     }
 #undef P
@@ -120,6 +124,10 @@ static int launch_op(const ds_plan_op& op, const unsigned char* gemm_kp, cudaStr
         case DS_OP_GEGLU: return ds_geglu_launch(&op.u.geglu, s);
         case DS_OP_GN_FINALIZE: return ds_gn_finalize_launch(&op.u.gn_finalize, s);
         case DS_OP_EMBED: return ds_embed_launch(&op.u.embed, s);
+        case DS_OP_OPT_PREP: return ds_opt_prep_launch(&op.u.opt_prep, s);
+        case DS_OP_OPT_SOFTMAX: return ds_opt_softmax_launch(&op.u.opt_softmax, s);
+        case DS_OP_OPT_REDUCE: return ds_opt_reduce_launch(&op.u.opt_reduce, s);
+        case DS_OP_OPT_KNN: return ds_opt_knn_launch(&op.u.opt_knn, s);
         case DS_OP_ATTN:
             if (gemm_kp) return dsb::attn_run(reinterpret_cast<const dsb::AttnKernelParams*>(gemm_kp), s);
             return ds_attn_launch(&op.u.attn, s);
@@ -459,6 +467,10 @@ size_t ds_sizeof(int which) {
         case DS_OP_GN_FINALIZE: return sizeof(ds_gn_finalize_desc);
         case DS_OP_ATTN: return sizeof(ds_attn_desc);
         case DS_OP_EMBED: return sizeof(ds_embed_desc);
+        case DS_OP_OPT_PREP: return sizeof(ds_opt_prep_desc);
+        case DS_OP_OPT_SOFTMAX: return sizeof(ds_opt_softmax_desc);
+        case DS_OP_OPT_REDUCE: return sizeof(ds_opt_reduce_desc);
+        case DS_OP_OPT_KNN: return sizeof(ds_opt_knn_desc);
         default: return 0;
     }
 }

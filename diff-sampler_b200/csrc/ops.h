@@ -346,6 +346,79 @@ typedef struct ds_gits_cost_desc {
 } ds_gits_cost_desc;
 
 int ds_gits_cost_launch(const ds_gits_cost_desc* d, cudaStream_t stream);
+
+// ---------------------------------------------------------------------------------------------
+// Optimal (empirical-Bayes) denoiser over a dataset y_0..y_{N-1} of D = C*H*W values each (optimal.cu; numerics in DESIGN.md 4.9):
+//   D*(x; sigma) = sum_i softmax_i(u_i / sigma^2) y_i,   u_i = x.y_i - 0.5 ||y_i||^2.
+// The two contractions run on the GEMM kernel (rows mode); these ops prepare and finish them.
+//
+// x [B][D] fp32 -> fp16 hi/lo planes [2][B][pitch] (columns D..pitch-1 zero) and ||x||^2 in fp64.
+typedef struct ds_opt_prep_desc {
+    const float* x;
+    void* planes;
+    double* xn2;            // [B]
+    int32_t B, D;
+    int32_t pitch, pad0;
+} ds_opt_prep_desc;
+
+// Row softmax of the logits GEMM.  part[s][b][i] (s < nslice, row pitch ldp) are the fp32 partials of x_b.y_i over channel slice s;
+// they are added in order s = 0, 1, ... in fp64, 0.5 ||y_i||^2 is subtracted, and u_i is kept in fp32 in slice 0.  Rows whose logit
+// error bound E_row exceeds DS_OPT_TAU and whose band (keys within 2 E_row + DS_OPT_BAND_NATS of the row maximum) holds at most
+// DS_OPT_CAP keys are rescored from exact fp32 distances; every other key then has weight 0.
+// P = 2^DS_OPT_P_SHIFT * softmax, as fp16 hi/lo planes [2][B][ldP] (columns N..ldP-1 zero).
+// status[b]: DS_OPT_PLAIN, DS_OPT_RESCORED, or DS_OPT_UNREFINED (E_row > tau but the band exceeded the cap).
+enum { DS_OPT_CAP = 1024, DS_OPT_P_SHIFT = 15, DS_OPT_BAND_NATS = 40 };
+#define DS_OPT_TAU 0.01f
+#define DS_OPT_EPS 7.62939453125e-06    /* 2^-17: relative error of u_i per ||x|| ||y_i|| (DESIGN.md 4.9) */
+enum { DS_OPT_PLAIN = 0, DS_OPT_RESCORED = 1, DS_OPT_UNREFINED = 2 };
+typedef struct ds_opt_softmax_desc {
+    float* part;
+    const double* hy2;      // [N] 0.5 ||y_i||^2 (fp64)
+    const double* xn2;      // [B] ||x_b||^2 (ds_opt_prep_desc)
+    const float* sigma;     // [nsig], nsig in {1, B}
+    const float* x;         // [B][D] fp32
+    const float* y;         // [N][D] fp32 dataset
+    void* P;
+    int32_t* status;        // [B], may be NULL
+    int64_t ldp, ldP;
+    int32_t B, N, D, nslice;
+    int32_t nsig;
+    float ymax;             // max_i ||y_i||
+} ds_opt_softmax_desc;
+
+// out[r][c] = scale * sum_{s < nsplit} part[s][r][c], s in increasing order: the split-K partials of the weighted-sum GEMM, rows of
+// pitch ld (a multiple of 4, for the GEMM epilogue's vector stores), into the dense [rows][cols] output (NCHW fp32).
+typedef struct ds_opt_reduce_desc {
+    const float* part;
+    float* out;
+    int64_t rows;
+    int32_t cols, ld;
+    int32_t nsplit;
+    float scale;
+} ds_opt_reduce_desc;
+
+// k nearest dataset rows of each x_b (k <= DS_KNN_MAX): candidates by u_i from the logits GEMM partials (as ds_opt_softmax_desc),
+// widened by the GEMM error bound, then exact distances ||x_b - y_i|| (fp32 differences, fp64 sums), ascending, ties to the lower
+// index.  dist [B][k] fp32, idx [B][k] int32.
+enum { DS_KNN_MAX = 64, DS_KNN_CAND = 256 };
+typedef struct ds_opt_knn_desc {
+    float* part;
+    const double* hy2;
+    const double* xn2;
+    const float* x;
+    const float* y;
+    float* dist;
+    int32_t* idx;
+    int64_t ldp;
+    int32_t B, N, D, nslice;
+    int32_t k;
+    float ymax;
+} ds_opt_knn_desc;
+
+int ds_opt_prep_launch(const ds_opt_prep_desc* d, cudaStream_t stream);
+int ds_opt_softmax_launch(const ds_opt_softmax_desc* d, cudaStream_t stream);
+int ds_opt_reduce_launch(const ds_opt_reduce_desc* d, cudaStream_t stream);
+int ds_opt_knn_launch(const ds_opt_knn_desc* d, cudaStream_t stream);
 int ds_amed_predict_launch(const float* w, const int* dims6, const float* bott, const float* t_cur, const float* t_next, float scale_dir,
                            float scale_time, float* out, int B, cudaStream_t stream);
 int ds_to_uint8_launch(const float* x, unsigned char* out, int B, int Cc, int HW, cudaStream_t stream);
@@ -371,7 +444,8 @@ int ds_embed_launch(const ds_embed_desc* d, cudaStream_t stream);
 //   bits 60..63 = space (0 absolute/NULL, 1 arena, 2 weights, 3 io slot), bits 0..59 = byte offset / slot.
 enum { DS_OP_GEMM = 1, DS_OP_GN_STATS = 2, DS_OP_GN_APPLY = 3, DS_OP_SOFTMAX = 4, DS_OP_POSEMB = 5, DS_OP_LINEAR = 6,
        DS_OP_PREP_INPUT = 7, DS_OP_CHANMEAN = 8, DS_OP_MEMSET = 9, DS_OP_LAYERNORM = 10, DS_OP_GEGLU = 11,
-       DS_OP_GN_FINALIZE = 12, DS_OP_ATTN = 13, DS_OP_EMBED = 14 };
+       DS_OP_GN_FINALIZE = 12, DS_OP_ATTN = 13, DS_OP_EMBED = 14, DS_OP_OPT_PREP = 15, DS_OP_OPT_SOFTMAX = 16,
+       DS_OP_OPT_REDUCE = 17, DS_OP_OPT_KNN = 18 };
 enum { DS_IO_X = 0, DS_IO_D = 1, DS_IO_SIGMA = 2, DS_IO_LABELS = 3, DS_IO_BOTTLENECK = 4, DS_IO_CTX = 5, DS_IO_COUNT = 6 };
 
 typedef struct ds_memset_desc {
@@ -397,6 +471,10 @@ typedef struct ds_plan_op {
         ds_gn_finalize_desc gn_finalize;
         ds_attn_desc attn;
         ds_embed_desc embed;
+        ds_opt_prep_desc opt_prep;
+        ds_opt_softmax_desc opt_softmax;
+        ds_opt_reduce_desc opt_reduce;
+        ds_opt_knn_desc opt_knn;
     } u;
 } ds_plan_op;
 

@@ -128,7 +128,7 @@ class PlanBuilder:
             desc = build(R)
             op.type = S.OP_TYPE_OF[type(desc)]
             op.tag = tag
-            setattr(op.u, S.UNION_FIELD[op.type], desc)
+            setattr(op.u, S.ALL_UNION_FIELD[op.type], desc)
         meta.update(n_ops=len(self.ops), n_gemm=sum(1 for op in arr if op.type == S.DS_OP_GEMM))
         return Plan(arr, len(self.ops), total, offsets, meta)
 

@@ -13,6 +13,7 @@ import torch
 from . import _cstructs as S
 from .ldm_net import B200LDMNet
 from .net import B200Net
+from .optimal import B200OptimalDenoiser, get_denoised_opt, optimal_sampler      # noqa: F401  (diff-analyzer's solvers.py)
 from .solver_utils import *                       # noqa: F401,F403  (the reference does `from solver_utils import *`)
 from .solver_utils import (dpm_pp_coefs, dyn_threshold, get_schedule, solver_update, unipc_coefs)
 
@@ -137,6 +138,8 @@ class _Loop:
         out = self.D if out is None else out
         if isinstance(net, B200Net):
             return net(x, sig, class_labels=self.kw['class_labels'], out=out)
+        if isinstance(net, B200OptimalDenoiser):
+            return net(x, sig, out=out)
         if isinstance(net, B200LDMNet):
             return net(x, sig, condition=self.kw['condition'], unconditional_condition=self.kw['unconditional_condition'], out=out)
         if hasattr(net, 'guidance_type'):
