@@ -14,7 +14,7 @@ EXPORTS = [
     'ds_version', 'ds_last_error', 'ds_weights_create', 'ds_weights_destroy', 'ds_unet_create', 'ds_unet_destroy',
     'ds_unet_forward', 'ds_unet_debug_read', 'ds_unet_last_launch_count', 'ds_solver_update', 'ds_dyn_threshold',
     'ds_op_launch', 'ds_sizeof', 'ds_unet_set_profiling', 'ds_unet_get_profile', 'ds_unet_op_type', 'ds_gits_cost', 'ds_unet_forward_io', 'ds_images_to_uint8', 'ds_solver_update_u8', 'ds_unet_enable_graph', 'ds_amed_predict',
-    'ds_gemm_config',
+    'ds_gemm_config', 'ds_op_check',
 ]
 
 _lib = None
@@ -59,6 +59,7 @@ def load():
     lib.ds_gits_cost.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int64, vp]
     lib.ds_images_to_uint8.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]
     lib.ds_op_launch.argtypes = [C.c_int, vp, sz, vp]
+    lib.ds_op_check.argtypes = [C.c_int, vp, sz]
     lib.ds_sizeof.argtypes = [C.c_int]
     lib.ds_sizeof.restype = sz
     lib.ds_gemm_config.argtypes = [vp, C.POINTER(C.c_int)]
@@ -84,6 +85,15 @@ def op_launch(desc, stream=0):
     """Launch one kernel-level op from a descriptor struct holding absolute device pointers."""
     lib = load()
     check(lib.ds_op_launch(S.OP_TYPE_OF[type(desc)], C.byref(desc), C.sizeof(desc), C.c_void_p(stream)), type(desc).__name__)
+
+
+def op_check(desc):
+    """None if the launcher of the descriptor's op accepts it, else the rule it breaks ("<op>: <rule>").  Needs no GPU; pointer fields
+    are only tested against NULL, so plan descriptors holding references are checked as they are."""
+    lib = load()
+    if lib.ds_op_check(S.OP_TYPE_OF[type(desc)], C.byref(desc), C.sizeof(desc)) == 0:
+        return None
+    return lib.ds_last_error().decode()
 
 
 def gemm_config(desc):

@@ -219,11 +219,17 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
 }
 
 // ------------------------------------------------------------------------------------------ host
+OpCheck attn_check(const ds_attn_desc& d) {
+    if (d.nplanes != 2 || d.B <= 0 || d.nh <= 0 || d.L <= 0 || d.Lk <= 0 || !(d.scale > 0.f)) return {-30, "attn: args"};
+    if (d.q_pitch % 8 || d.k_pitch % 8 || d.vt_pitch % 8 || d.o_pitch % 8 || d.q_c0 % 8 || d.k_c0 % 8) return {-31, "attn: pitch"};
+    if (d.q_c0 + d.nh * 64 > d.q_pitch || d.k_c0 + d.nh * 64 > d.k_pitch || d.nh * 64 > d.o_pitch || d.Lk > d.vt_pitch)
+        return {-32, "attn: extent"};
+    if (d.causal && d.L != d.Lk) return {-40, "attn: causal"};        // the causal mask is defined for self-attention only
+    return {0, nullptr};
+}
+
 int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
-    if (d->nplanes != 2 || d->B <= 0 || d->nh <= 0 || d->L <= 0 || d->Lk <= 0 || !(d->scale > 0.f)) return -30;
-    if (d->q_pitch % 8 || d->k_pitch % 8 || d->vt_pitch % 8 || d->o_pitch % 8 || d->q_c0 % 8 || d->k_c0 % 8) return -31;
-    if (d->q_c0 + d->nh * 64 > d->q_pitch || d->k_c0 + d->nh * 64 > d->k_pitch || d->nh * 64 > d->o_pitch || d->Lk > d->vt_pitch) return -32;
-    if (d->causal && d->L != d->Lk) return -40;                       // the causal mask is defined for self-attention only
+    if (const int rc = attn_check(*d).rc) return rc;
     {
         const int64_t dims[3] = {d->q_pitch, d->L, (int64_t)2 * d->B};
         const int64_t str[2] = {(int64_t)d->q_pitch * 2, (int64_t)d->L * d->q_pitch * 2};

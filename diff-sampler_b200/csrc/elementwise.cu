@@ -770,11 +770,17 @@ static inline int ok() { return cudaGetLastError() == cudaSuccess ? 0 : -1; }
 
 using namespace dsb;
 
-extern "C" int ds_gn_stats_launch(const ds_gn_stats_desc* d, cudaStream_t stream) {
-    const int C = d->C0 + d->C1;
-    if (C % 4 || d->groups <= 0 || d->groups > 64 || C % d->groups || (d->C0 % 4)) return -2;
+OpCheck dsb::gn_stats_check(const ds_gn_stats_desc& d) {
+    const int C = d.C0 + d.C1;
+    if (C % 4 || d.groups <= 0 || d.groups > 64 || C % d.groups || (d.C0 % 4)) return {-2, "gn_stats: channels"};
     // gn_stats_kernel splits a float4 column between at most two groups (gA / gB): groups of one channel would be summed into the wrong group
-    if (C / d->groups < 2) return -2;
+    if (C / d.groups < 2) return {-2, "gn_stats: one-channel groups"};
+    return {0, nullptr};
+}
+
+extern "C" int ds_gn_stats_launch(const ds_gn_stats_desc* d, cudaStream_t stream) {
+    if (const int rc = gn_stats_check(*d).rc) return rc;
+    const int C = d->C0 + d->C1;
     const int ncol4 = C / 4;
     int bx = ncol4 < 256 ? ncol4 : 256;
     // keep bx a divisor-friendly size; columns loop with stride bx anyway
@@ -789,45 +795,67 @@ extern "C" int ds_gn_stats_launch(const ds_gn_stats_desc* d, cudaStream_t stream
     return ok();
 }
 
-extern "C" int ds_gn_finalize_launch(const ds_gn_finalize_desc* d, cudaStream_t stream) {
-    const int C = d->C0 + d->C1;
-    if (d->groups <= 0 || d->groups > 64 || C % d->groups) return -2;
-    if (d->quads0) {
-        const int u0 = d->unit0 == 2 ? 2 : 4, u1 = d->unit1 == 2 ? 2 : 4;
-        const int cpg = C / d->groups;
-        if (d->C0 % u0 || d->C1 % u1 || (d->C1 > 0 && !d->quads1)) return -2;
+// Block size and dynamic shared memory of gn_finalize_kernel.  threads: enough for (columns x slab groups), at most 1024; shared memory:
+// [cols] + [SG][cols] doubles, cols <= C, SG * cols <= max(cols, threads)
+static size_t gn_finalize_shape(const ds_gn_finalize_desc& d, int* threads) {
+    *threads = 256;
+    if (!d.quads0) return (size_t)(d.C0 + d.C1 + 2) * sizeof(double);
+    const int u0 = d.unit0 == 2 ? 2 : 4, u1 = d.unit1 == 2 ? 2 : 4;
+    const int cols = d.C0 / u0 * 2 + d.C1 / u1 * 2;
+    *threads = 1024;
+    const int sg = cols >= *threads ? 1 : *threads / cols;
+    return (size_t)(cols + (size_t)sg * cols + 2) * sizeof(double);
+}
+
+OpCheck dsb::gn_finalize_check(const ds_gn_finalize_desc& d) {
+    const int C = d.C0 + d.C1;
+    if (d.groups <= 0 || d.groups > 64 || C % d.groups) return {-2, "gn_finalize: groups"};
+    if (d.quads0) {
+        const int u0 = d.unit0 == 2 ? 2 : 4, u1 = d.unit1 == 2 ? 2 : 4;
+        const int cpg = C / d.groups;
+        if (d.C0 % u0 || d.C1 % u1 || (d.C1 > 0 && !d.quads1)) return {-2, "gn_finalize: source units"};
         // every group must be a union of whole partial units of the sources it covers
-        const int rem = d->C0 % cpg;                    // channels of a group that straddles the two sources, on the source-0 side
-        if (cpg % u0 || rem % u0) return -2;
-        if (d->C1 > 0 && (cpg % u1 || (rem ? (cpg - rem) % u1 : 0))) return -2;
+        const int rem = d.C0 % cpg;                     // channels of a group that straddles the two sources, on the source-0 side
+        if (cpg % u0 || rem % u0) return {-2, "gn_finalize: group units"};
+        if (d.C1 > 0 && (cpg % u1 || (rem ? (cpg - rem) % u1 : 0))) return {-2, "gn_finalize: group units"};
     }
-    if (!d->quads0 && !d->coef) return -2;               // nothing to do
-    if (d->coef && (!d->gamma || !d->beta || d->HW <= 0)) return -2;
-    // threads: enough for (columns x slab groups), at most 1024; shared memory: [cols] + [SG][cols] doubles, cols <= C, SG * cols <= max(cols, threads)
-    int threads = 256;
-    size_t smem = (size_t)(C + 2) * sizeof(double);
-    if (d->quads0) {
-        const int u0 = d->unit0 == 2 ? 2 : 4, u1 = d->unit1 == 2 ? 2 : 4;
-        const int cols = d->C0 / u0 * 2 + d->C1 / u1 * 2;
-        threads = 1024;
-        const int sg = cols >= threads ? 1 : threads / cols;
-        smem = (size_t)(cols + (size_t)sg * cols + 2) * sizeof(double);
-    }
+    if (!d.quads0 && !d.coef) return {-2, "gn_finalize: nothing to do"};
+    if (d.coef && (!d.gamma || !d.beta || d.HW <= 0)) return {-2, "gn_finalize: coef inputs"};
+    // the launch keeps the default 48 KiB limit of dynamic shared memory
+    int threads;
+    if (gn_finalize_shape(d, &threads) > 48 * 1024) return {-2, "gn_finalize: shared memory"};
+    return {0, nullptr};
+}
+
+extern "C" int ds_gn_finalize_launch(const ds_gn_finalize_desc* d, cudaStream_t stream) {
+    if (const int rc = gn_finalize_check(*d).rc) return rc;
+    int threads;
+    const size_t smem = gn_finalize_shape(*d, &threads);
     gn_finalize_kernel<<<d->B, threads, smem, stream>>>(*d);
     return ok();
 }
 
-extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream) {
-    const int C = d->C0 + d->C1;
-    if (C % 8 || (d->C0 % 8)) return -2;
-    if (d->fmt != 0 && (d->fmt != 1 || d->resample == 3 || d->nplanes != 2)) return -2;   // the f8 layout reuses the two-plane footprint
+OpCheck dsb::gn_apply_check(const ds_gn_apply_desc& d) {
+    const int C = d.C0 + d.C1;
+    if (C % 8 || (d.C0 % 8)) return {-2, "gn_apply: channels"};
+    // the f8 layout reuses the two-plane footprint
+    if (d.fmt != 0 && (d.fmt != 1 || d.resample == 3 || d.nplanes != 2)) return {-2, "gn_apply: fmt"};
     // the coefficient table is read by the resample-0 kernel only; the resampling kernels normalise from the sums
-    if (d->coef && d->resample != 0) return -2;
-    if (d->out_act && !d->sums && !d->coef) return -2;                                      // a normalised output needs statistics
+    if (d.coef && d.resample != 0) return {-2, "gn_apply: coef with resample"};
+    if (d.out_act && !d.sums && !d.coef) return {-2, "gn_apply: statistics"};          // a normalised output needs statistics
     // 2x2 pooling and space-to-depth take whole 2x2 blocks: an odd row or column has no output pixel
-    if ((d->resample == 1 || d->resample == 3) && (d->H % 2 || d->W % 2)) return -2;
+    if ((d.resample == 1 || d.resample == 3) && (d.H % 2 || d.W % 2)) return {-2, "gn_apply: resample parity"};
     const int nc8 = C / 8;
-    if (nc8 > 512) return -2;
+    if (nc8 > 512) return {-2, "gn_apply: width"};                                   // at most 4096 channels
+    // the persistent kernel takes at most 256 threads (2048 channels); wider tensors use the sums path
+    if (d.coef && d.resample == 0 && d.sums == nullptr && nc8 > 256) return {-2, "gn_apply: coef width"};
+    return {0, nullptr};
+}
+
+extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream) {
+    if (const int rc = gn_apply_check(*d).rc) return rc;
+    const int C = d->C0 + d->C1;
+    const int nc8 = C / 8;
     int rows = 256 / nc8;
     if (rows < 1) rows = 1;
     const int threads = nc8 * rows;
@@ -839,7 +867,6 @@ extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream
     while (pix_per_cta > rows && (long long)((npix + pix_per_cta - 1) / pix_per_cta) * d->B < 132 * 4) pix_per_cta /= 2;
     const int chunks = (npix + pix_per_cta - 1) / pix_per_cta;
     dim3 grid(chunks, d->B);
-    if (d->coef && d->resample == 0 && d->sums == nullptr && threads > 256) return -2;      // wider than 2048 channels: use the sums path
     if (d->coef && d->resample == 0 && d->sums == nullptr) {
         // persistent variant: grid = co-resident CTAs (occupancy query per block size and device, cached)
         static int occ[64][17] = {};
@@ -870,19 +897,29 @@ extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream
     return ok();
 }
 
+OpCheck dsb::embed_check(const ds_embed_desc& d) {
+    if (d.C % 4 || d.rows <= 0 || d.T <= 0 || d.vocab <= 0) return {-2, "embed: shape"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_embed_launch(const ds_embed_desc* d, cudaStream_t stream) {
-    if (d->C % 4 || d->rows <= 0 || d->T <= 0 || d->vocab <= 0) return -2;
+    if (const int rc = embed_check(*d).rc) return rc;
     const long long total = d->rows * (d->C / 4);
     embed_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(*d);
     return ok();
 }
 
+OpCheck dsb::layernorm_check(const ds_layernorm_desc& d) {
+    if (d.C % 4 || d.C > 2048) return {-2, "layernorm: C"};
+    if (d.fmt == 1 && d.nplanes != 2) return {-2, "layernorm: f8 planes"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_layernorm_launch(const ds_layernorm_desc* d, cudaStream_t stream) {
-    if (d->C % 4 || d->C > 2048) return -2;
+    if (const int rc = layernorm_check(*d).rc) return rc;
     const int wpb = 8;
     const unsigned blocks = (unsigned)((d->rows + wpb - 1) / wpb);
     if (d->fmt == 1) {
-        if (d->nplanes != 2) return -2;
         layernorm_kernel<1><<<blocks, wpb * 32, 0, stream>>>(*d);
     } else if (d->fmt == 2) {
         layernorm_kernel<2><<<blocks, wpb * 32, 0, stream>>>(*d);
@@ -892,14 +929,19 @@ extern "C" int ds_layernorm_launch(const ds_layernorm_desc* d, cudaStream_t stre
     return ok();
 }
 
+OpCheck dsb::geglu_check(const ds_geglu_desc& d) {
+    if (d.I % 4) return {-2, "geglu: I"};
+    if (d.mode == 1 && d.fmt != 0) return {-2, "geglu: quick-GELU fmt"};
+    if (d.mode != 1 && d.fmt == 1 && d.nplanes != 2) return {-2, "geglu: f8 planes"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_geglu_launch(const ds_geglu_desc* d, cudaStream_t stream) {
-    if (d->I % 4) return -2;
+    if (const int rc = geglu_check(*d).rc) return rc;
     const unsigned blocks = (unsigned)((d->rows * (d->I / 4) + 255) / 256);
     if (d->mode == 1) {
-        if (d->fmt != 0) return -2;
         gate_kernel<1, 0><<<blocks, 256, 0, stream>>>(*d);
     } else if (d->fmt == 1) {
-        if (d->nplanes != 2) return -2;
         gate_kernel<0, 1><<<blocks, 256, 0, stream>>>(*d);
     } else {
         gate_kernel<0, 0><<<blocks, 256, 0, stream>>>(*d);
@@ -931,7 +973,13 @@ extern "C" int ds_posemb_launch(const ds_posemb_desc* d, cudaStream_t stream) {
     return ok();
 }
 
+OpCheck dsb::linear_check(const ds_linear_desc& d) {
+    if (d.in_f > 2048) return {-2, "linear: in_f"};            // the widest kernel holds 2048 weights of a row in registers
+    return {0, nullptr};
+}
+
 extern "C" int ds_linear_launch(const ds_linear_desc* d, cudaStream_t stream) {
+    if (const int rc = linear_check(*d).rc) return rc;
     const int wpb = 4;
     const int bx = (d->out_f + wpb - 1) / wpb;
     int by = d->n_rows < 16 ? d->n_rows : 16;
@@ -939,15 +987,19 @@ extern "C" int ds_linear_launch(const ds_linear_desc* d, cudaStream_t stream) {
     if (d->in_f <= 256) linear_kernel<256><<<dim3(bx, by), wpb * 32, 0, stream>>>(*d);
     else if (d->in_f <= 512) linear_kernel<512><<<dim3(bx, by), wpb * 32, 0, stream>>>(*d);
     else if (d->in_f <= 1024) linear_kernel<1024><<<dim3(bx, by), wpb * 32, 0, stream>>>(*d);
-    else if (d->in_f <= 2048) linear_kernel<2048><<<dim3(bx, by), wpb * 32, 0, stream>>>(*d);
-    else return -2;
+    else linear_kernel<2048><<<dim3(bx, by), wpb * 32, 0, stream>>>(*d);
     return ok();
 }
 
+OpCheck dsb::prep_input_check(const ds_prep_input_desc& d) {
+    if (d.C > 64) return {-2, "prep_input: C"};
+    if (d.codebook && (d.C > 8 || d.n_embed < 1)) return {-2, "prep_input: codebook"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_prep_input_launch(const ds_prep_input_desc* d, cudaStream_t stream) {
-    if (d->C > 64) return -2;
+    if (const int rc = prep_input_check(*d).rc) return rc;
     if (d->codebook) {
-        if (d->C > 8 || d->n_embed < 1) return -2;
         const unsigned blocks = (unsigned)(((long long)d->B * d->HW + 255) / 256);
         if (d->C <= 4) vq_prep_input_kernel<4><<<blocks, 256, 0, stream>>>(*d);
         else vq_prep_input_kernel<8><<<blocks, 256, 0, stream>>>(*d);

@@ -108,6 +108,28 @@ static void visit_ptrs(ds_plan_op& op, F f) {
 #undef P
 }
 
+// The launcher's descriptor check of the op (ops.h).  Posemb, softmax, chanmean and memset accept every descriptor.
+static dsb::OpCheck check_op(const ds_plan_op& op) {
+    switch (op.type) {
+        case DS_OP_GEMM: return dsb::gemm_check(op.u.gemm);
+        case DS_OP_GN_STATS: return dsb::gn_stats_check(op.u.gn_stats);
+        case DS_OP_GN_APPLY: return dsb::gn_apply_check(op.u.gn_apply);
+        case DS_OP_LINEAR: return dsb::linear_check(op.u.linear);
+        case DS_OP_PREP_INPUT: return dsb::prep_input_check(op.u.prep_input);
+        case DS_OP_LAYERNORM: return dsb::layernorm_check(op.u.layernorm);
+        case DS_OP_GEGLU: return dsb::geglu_check(op.u.geglu);
+        case DS_OP_GN_FINALIZE: return dsb::gn_finalize_check(op.u.gn_finalize);
+        case DS_OP_ATTN: return dsb::attn_check(op.u.attn);
+        case DS_OP_EMBED: return dsb::embed_check(op.u.embed);
+        case DS_OP_OPT_PREP: return dsb::opt_prep_check(op.u.opt_prep);
+        case DS_OP_OPT_SOFTMAX: return dsb::opt_softmax_check(op.u.opt_softmax);
+        case DS_OP_OPT_REDUCE: return dsb::opt_reduce_check(op.u.opt_reduce);
+        case DS_OP_OPT_KNN: return dsb::opt_knn_check(op.u.opt_knn);
+        case DS_OP_SOFTMAX: case DS_OP_POSEMB: case DS_OP_CHANMEAN: case DS_OP_MEMSET: return {0, nullptr};
+        default: return {-100, "unknown op type"};
+    }
+}
+
 static int launch_op(const ds_plan_op& op, const unsigned char* gemm_kp, cudaStream_t s) {
     switch (op.type) {
         case DS_OP_GEMM:
@@ -171,6 +193,16 @@ int ds_unet_create(const ds_weights* w, const void* plan_ops, int n_ops, size_t 
         char buf[128];
         snprintf(buf, sizeof buf, "ds_unet_create: ds_plan_op size mismatch (caller %zu, library %zu)", op_size, sizeof(ds_plan_op));
         return fail(-4, buf);
+    }
+    // refuse a plan with an op its launcher would refuse before anything is allocated (the checks hold on pointer references)
+    for (int i = 0; i < n_ops; ++i) {
+        const ds_plan_op& op = reinterpret_cast<const ds_plan_op*>(plan_ops)[i];
+        const dsb::OpCheck c = check_op(op);
+        if (c.rc) {
+            char buf[160];
+            snprintf(buf, sizeof buf, "ds_unet_create: op %d (type %d tag %d) refused (rc %d): %s", i, op.type, op.tag, c.rc, c.rule);
+            return fail(-6, buf);
+        }
     }
     ds_unet* u = new ds_unet();
     u->w = w;
@@ -512,6 +544,16 @@ int ds_op_launch(int op_type, const void* desc, size_t desc_size, void* stream) 
         return fail(rc, buf);
     }
     return 0;
+}
+
+int ds_op_check(int op_type, const void* desc, size_t desc_size) {
+    ds_plan_op op;
+    memset(&op, 0, sizeof op);
+    op.type = op_type;
+    if (desc_size > sizeof(op.u)) return fail(-1, "ds_op_check: descriptor too large");
+    memcpy(&op.u, desc, desc_size);
+    const dsb::OpCheck c = check_op(op);
+    return c.rc ? fail(c.rc, c.rule) : 0;
 }
 
 }  // extern "C"

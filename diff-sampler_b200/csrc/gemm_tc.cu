@@ -603,11 +603,32 @@ int encode_map(CUtensorMap* m, const void* ptr, int rank, const int64_t* dims, c
     return encode_map_typed(m, ptr, rank, dims, strides_bytes, box, false);
 }
 
+OpCheck gemm_check(const ds_gemm_desc& d) {
+    if (d.BN < 16 || d.BN > 256 || (d.BN % 16) != 0) return {-10, "gemm: BN"};
+    // A conv box of whole image rows (a_box[1] == conv_W <= 128) holds 128 pixels only when conv_W divides 128
+    if (d.a_box[0] != 64 || d.a_box[1] * d.a_box[2] * d.a_box[3] != 128) return {-11, "gemm: a_box"};
+    if (d.npass != 1 && d.npass != 3) return {-12, "gemm: npass"};
+    // cuTensorMapEncodeTiled limits of the A map (what its failed encode returns): extents <= 2^32, strides multiples of 16 below 2^40
+    for (int i = 0; i < 4; ++i) if (d.a_dims[i] > (int64_t(1) << 32)) return {-1, "gemm: A tensor map"};
+    for (int i = 0; i < 3; ++i) if (d.a_strides[i] % 16 || d.a_strides[i] >= (int64_t(1) << 40)) return {-1, "gemm: A tensor map"};
+    if (d.st_unit != 0 && d.st_unit != 2 && d.st_unit != 4) return {-14, "gemm: st_unit"};
+    if (d.f8 & 1) {
+        // e4m3 correction passes: conv mode, one z slice, three passes, a lo plane; the byte planes have no phase channel bases
+        if (d.a_mode != 0 || d.num_z != 1 || d.npass != 3 || d.a_plane_n <= 0) return {-16, "gemm: f8"};
+        for (int t = 0; t < 9; ++t) if (d.tap_cb[t]) return {-16, "gemm: f8 with tap_cb"};
+    }
+    if (d.taps != 1 && d.taps != 9) return {-15, "gemm: taps"};
+    // image rows wider than one M tile: the tile is a 128-pixel segment of one row
+    if (d.a_mode == 0 && d.conv_W > 128 && (d.conv_W % 128 != 0 || d.a_box[1] != 128)) return {-13, "gemm: row segment"};
+    // fused statistics: whole 32-row slabs (row validity is then warp-uniform), whole channel quads, one z slice, fp32 output
+    if (d.st_quads && (d.num_z != 1 || d.m_valid % 32 != 0 || d.n_valid % (d.st_unit == 2 ? 2 : 4) != 0 || d.edm_out != 0))
+        return {-14, "gemm: st_quads"};
+    return {0, nullptr};
+}
+
 int gemm_build(const ds_gemm_desc* d, GemmKernelParams* kp) {
     memset(kp, 0, sizeof(*kp));
-    if (d->BN < 16 || d->BN > 256 || (d->BN % 16) != 0) return -10;
-    if (d->a_box[0] != 64 || d->a_box[1] * d->a_box[2] * d->a_box[3] != 128) return -11;
-    if (d->npass != 1 && d->npass != 3) return -12;
+    if (const int rc = gemm_check(*d).rc) return rc;
     if (encode_map(&kp->tmA, d->a_ptr, 4, d->a_dims, d->a_strides, d->a_box)) return -1;
     if (d->a2_c > 0) {
         int64_t dims2[4] = {d->a2_c, d->a_dims[1], d->a_dims[2], d->a_dims[3]};
@@ -635,12 +656,9 @@ int gemm_build(const ds_gemm_desc* d, GemmKernelParams* kp) {
     kp->edm_C = d->edm_C; kp->edm_D = d->edm_D;
     kp->st_quads = d->st_quads;
     kp->st_unit = d->st_unit == 2 ? 2 : 4;
-    if (d->st_unit != 0 && d->st_unit != 2 && d->st_unit != 4) return -14;
     kp->acc_scale = d->acc_scale == 0.f ? 1.f : d->acc_scale;
     if (d->f8 & 1) {
         // e4m3 correction passes: byte planes behind the fp16 plane of each operand (layout: csrc/ops.h)
-        if (d->a_mode != 0 || d->num_z != 1 || d->npass != 3 || d->a_plane_n <= 0) return -16;
-        for (int t = 0; t < 9; ++t) if (d->tap_cb[t]) return -16;
         const int64_t C = d->a_dims[0], Wd = d->a_dims[1], Hd = d->a_dims[2], Bn = d->a_plane_n;
         const int32_t box8[4] = {128, d->a_box[1], d->a_box[2], d->a_box[3]};
         const int64_t dims8[4] = {C, Wd, Hd, 2 * Bn};
@@ -670,11 +688,6 @@ int gemm_build(const ds_gemm_desc* d, GemmKernelParams* kp) {
         if (encode_map_typed(&kp->tmB8, b8, 3, bd8, bs8, bbox8, true)) return -19;
     }
     for (int t = 0; t < 9; ++t) { kp->tap_dh[t] = d->tap_dh[t]; kp->tap_dw[t] = d->tap_dw[t]; kp->tap_cb[t] = d->tap_cb[t]; }
-    if (d->taps != 1 && d->taps != 9) return -15;
-    // image rows wider than one M tile: the tile is a 128-pixel segment of one row
-    if (d->a_mode == 0 && d->conv_W > 128 && (d->conv_W % 128 != 0 || d->a_box[1] != 128)) return -13;
-    // fused statistics: whole 32-row slabs (row validity is then warp-uniform), whole channel quads, one z slice, fp32 output
-    if (d->st_quads && (d->num_z != 1 || d->m_valid % 32 != 0 || d->n_valid % (d->st_unit == 2 ? 2 : 4) != 0 || d->edm_out != 0)) return -14;
     const int stage_bytes = kATileBytes + d->BN * 128;
     int ns = (kSmemLimit - 1024 - kStgBytes - (int)sizeof(SmemCtl)) / stage_bytes;
     if (ns > kMaxStages) ns = kMaxStages;

@@ -480,4 +480,28 @@ typedef struct ds_plan_op {
 
 #ifdef __cplusplus
 }
+
+namespace dsb {
+// The descriptor rules of each launcher, one check per op type next to its launcher, run first by the launcher, by ds_op_check and, on
+// every op of a plan, by ds_unet_create.  rc is 0 or the code the launcher returns; rule names the broken rule ("<op>: <rule>").  Pure
+// host functions: no CUDA call, and pointers are only tested against NULL, so they hold for plan references as for device addresses.
+struct OpCheck {
+    int rc;
+    const char* rule;
+};
+OpCheck gemm_check(const ds_gemm_desc& d);
+OpCheck attn_check(const ds_attn_desc& d);
+OpCheck gn_stats_check(const ds_gn_stats_desc& d);
+OpCheck gn_finalize_check(const ds_gn_finalize_desc& d);
+OpCheck gn_apply_check(const ds_gn_apply_desc& d);
+OpCheck embed_check(const ds_embed_desc& d);
+OpCheck layernorm_check(const ds_layernorm_desc& d);
+OpCheck geglu_check(const ds_geglu_desc& d);
+OpCheck linear_check(const ds_linear_desc& d);
+OpCheck prep_input_check(const ds_prep_input_desc& d);
+OpCheck opt_prep_check(const ds_opt_prep_desc& d);
+OpCheck opt_softmax_check(const ds_opt_softmax_desc& d);
+OpCheck opt_reduce_check(const ds_opt_reduce_desc& d);
+OpCheck opt_knn_check(const ds_opt_knn_desc& d);
+}  // namespace dsb
 #endif

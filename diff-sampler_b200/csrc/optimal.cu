@@ -239,28 +239,50 @@ __global__ void __launch_bounds__(kOptThreads) opt_knn_kernel(ds_opt_knn_desc d)
 
 }  // namespace dsb
 
+dsb::OpCheck dsb::opt_prep_check(const ds_opt_prep_desc& d) {
+    if (d.B <= 0 || d.D <= 0 || d.pitch < d.D || (d.pitch & 7)) return {-1, "opt_prep: shape"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_opt_prep_launch(const ds_opt_prep_desc* d, cudaStream_t stream) {
-    if (d->B <= 0 || d->D <= 0 || d->pitch < d->D || (d->pitch & 7)) return -1;
+    if (const int rc = dsb::opt_prep_check(*d).rc) return rc;
     dsb::opt_prep_kernel<<<d->B, 256, 0, stream>>>(*d);
     return dsb::opt_ok();
 }
 
+dsb::OpCheck dsb::opt_softmax_check(const ds_opt_softmax_desc& d) {
+    if (d.B <= 0 || d.N <= 0 || d.nslice <= 0 || d.ldp < d.N || d.ldP < d.N) return {-1, "opt_softmax: shape"};
+    if (d.nsig != 1 && d.nsig != d.B) return {-1, "opt_softmax: nsig"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_opt_softmax_launch(const ds_opt_softmax_desc* d, cudaStream_t stream) {
-    if (d->B <= 0 || d->N <= 0 || d->nslice <= 0 || d->ldp < d->N || d->ldP < d->N || (d->nsig != 1 && d->nsig != d->B)) return -1;
+    if (const int rc = dsb::opt_softmax_check(*d).rc) return rc;
     dsb::opt_softmax_kernel<<<d->B, dsb::kOptThreads, 0, stream>>>(*d);
     return dsb::opt_ok();
 }
 
+dsb::OpCheck dsb::opt_reduce_check(const ds_opt_reduce_desc& d) {
+    if (d.rows <= 0 || d.cols <= 0 || d.ld < d.cols || d.nsplit <= 0) return {-1, "opt_reduce: shape"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_opt_reduce_launch(const ds_opt_reduce_desc* d, cudaStream_t stream) {
-    if (d->rows <= 0 || d->cols <= 0 || d->ld < d->cols || d->nsplit <= 0) return -1;
+    if (const int rc = dsb::opt_reduce_check(*d).rc) return rc;
     long long blocks = (d->rows * d->cols + 255) / 256;
     if (blocks > 132 * 8) blocks = 132 * 8;
     dsb::opt_reduce_kernel<<<(unsigned)blocks, 256, 0, stream>>>(*d);
     return dsb::opt_ok();
 }
 
+dsb::OpCheck dsb::opt_knn_check(const ds_opt_knn_desc& d) {
+    if (d.B <= 0 || d.N <= 0 || d.ldp < d.N) return {-1, "opt_knn: shape"};
+    if (d.k <= 0 || d.k > DS_KNN_MAX || d.k > d.N) return {-1, "opt_knn: k"};
+    return {0, nullptr};
+}
+
 extern "C" int ds_opt_knn_launch(const ds_opt_knn_desc* d, cudaStream_t stream) {
-    if (d->B <= 0 || d->N <= 0 || d->k <= 0 || d->k > DS_KNN_MAX || d->k > d->N || d->ldp < d->N) return -1;
+    if (const int rc = dsb::opt_knn_check(*d).rc) return rc;
     dsb::opt_knn_kernel<<<d->B, dsb::kOptThreads, 0, stream>>>(*d);
     return dsb::opt_ok();
 }

@@ -117,6 +117,10 @@ int ds_images_to_uint8(const float* images, unsigned char* out, int B, int C, in
 /* ---- kernel-level entry points (used by the parity tests and micro-benchmarks) ------------------
  * `desc` points to the matching struct of csrc/ops.h with absolute device pointers. */
 int ds_op_launch(int op_type, const void* desc, size_t desc_size, void* stream);
+/* The descriptor check ds_op_launch's launcher runs first, without launching: 0, or the code the launcher would return with
+ * "<op>: <rule>" in ds_last_error().  Needs no GPU; pointers are only tested against NULL.  ds_unet_create checks every op of a plan
+ * this way before it allocates anything. */
+int ds_op_check(int op_type, const void* desc, size_t desc_size);
 /* sizeof() of the descriptor structs as compiled (0 = ds_plan_op, else DS_OP_* code); lets bindings verify their mirrors. */
 size_t ds_sizeof(int which);
 /* How the GEMM kernel would run `desc` (a ds_gemm_desc) on the current device: info[0] shared-memory ring stages, info[1] CTAs in

@@ -1,6 +1,6 @@
 """Consistency-Models LSUN-256 nets (lsun_bedroom, lsun_cat) on the host: the float64 oracle against the real reference
 (tests/golden/ref_cm.npz, oracle/gen_cm_golden.py), the importer's structure at the full lsun_setting, the qkv row permutation,
-the tiny CM plan on the CPU plan interpreter, the launcher argument checks over the full-size plan, and the other plan kinds
+the tiny CM plan on the CPU plan interpreter, the launchers' descriptor checks over the full-size plan, and the other plan kinds
 compiling byte for byte as before."""
 import json
 import os
@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from diff_sampler_b200 import _cstructs as S
+from diff_sampler_b200 import _lib
 from diff_sampler_b200 import cm_net, gemm_desc as G, plan as planner
 from oracle import cm_interp as CI
 from oracle import cm_oracle as CO
@@ -132,83 +133,17 @@ def test_cm_plan_on_the_cpu_interpreter(ref, tiny, f8):
         assert err_tap < TOL[f8] * max(1.0, tap.abs().max().item())
 
 
-def _launcher_guard(op):
-    """The argument checks of the op's launcher that do not need a device (csrc/gemm_tc.cu gemm_build, csrc/elementwise.cu
-    ds_gn_*_launch / ds_linear_launch / ds_prep_input_launch, csrc/attention.cu); returns the failing check or None."""
-    t, d = op.type, getattr(op.u, S.UNION_FIELD[op.type])
-    if t == S.DS_OP_GEMM:
-        if d.BN < 16 or d.BN > 256 or d.BN % 16:
-            return 'BN'
-        if d.a_box[0] != 64 or d.a_box[1] * d.a_box[2] * d.a_box[3] != 128:
-            return 'a_box'
-        if d.taps not in (1, 9):
-            return 'taps'
-        if d.a_mode == 0 and d.conv_W > 128 and (d.conv_W % 128 or d.a_box[1] != 128):
-            return 'row segment'
-        if d.st_quads and (d.num_z != 1 or d.m_valid % 32 or d.n_valid % (2 if d.st_unit == 2 else 4) or d.edm_out):
-            return 'st_quads'
-        if d.f8 and (d.a_mode != 0 or d.num_z != 1 or d.npass != 3 or d.a_plane_n <= 0):
-            return 'f8'
-        if any(int(x) >= 1 << 32 for x in d.a_dims) or any(int(s) % 16 or int(s) >= 1 << 40 for s in d.a_strides):
-            return 'A tensor map'
-        if d.a_mode == 0 and d.conv_W <= 128 and 128 % d.conv_W:
-            return 'conv width'
-    elif t == S.DS_OP_GN_APPLY:
-        C = d.C0 + d.C1
-        nc8 = C // 8
-        if C % 8 or d.C0 % 8 or nc8 > 512:
-            return 'channels'
-        if d.coef and d.resample == 0 and not d.sums and nc8 * max(1, 256 // nc8) > 256:
-            return 'coef width'
-        if d.coef and d.resample != 0:
-            return 'coef resample'
-        if d.out_act and not d.sums and not d.coef:
-            return 'statistics'
-        if d.resample in (1, 3) and (d.H % 2 or d.W % 2):
-            return 'resample parity'
-    elif t == S.DS_OP_GN_STATS:
-        C = d.C0 + d.C1
-        if C % 4 or d.groups <= 0 or d.groups > 64 or C % d.groups or d.C0 % 4 or C // d.groups < 2:
-            return 'channels'
-    elif t == S.DS_OP_GN_FINALIZE:
-        C = d.C0 + d.C1
-        if d.groups <= 0 or d.groups > 64 or C % d.groups:
-            return 'groups'
-        if d.quads0:
-            u0, u1 = (2 if d.unit0 == 2 else 4), (2 if d.unit1 == 2 else 4)
-            cpg, rem = C // d.groups, d.C0 % (C // d.groups)
-            if d.C0 % u0 or d.C1 % u1 or (d.C1 and not d.quads1) or cpg % u0 or rem % u0:
-                return 'units'
-            if d.C1 and (cpg % u1 or (rem and (cpg - rem) % u1)):
-                return 'units'
-            cols = d.C0 // u0 * 2 + d.C1 // u1 * 2
-            if (cols + max(1, 1024 // cols) * cols + 2) * 8 > 48 * 1024:
-                return 'shared memory'
-        if not d.quads0 and not d.coef:
-            return 'nothing to do'
-        if d.coef and (not d.gamma or not d.beta or d.HW <= 0):
-            return 'coef'
-    elif t == S.DS_OP_LINEAR:
-        if d.in_f > 2048:
-            return 'in_f'
-    elif t == S.DS_OP_PREP_INPUT:
-        if d.C > 64:
-            return 'C'
-    elif t == S.DS_OP_ATTN:
-        if d.nplanes != 2 or min(d.B, d.nh, d.L, d.Lk) <= 0 or not d.scale > 0:
-            return 'args'
-        if d.q_pitch % 8 or d.k_pitch % 8 or d.vt_pitch % 8 or d.o_pitch % 8 or d.q_c0 % 8 or d.k_c0 % 8:
-            return 'pitch'
-        if d.q_c0 + d.nh * 64 > d.q_pitch or d.k_c0 + d.nh * 64 > d.k_pitch or d.nh * 64 > d.o_pitch or d.Lk > d.vt_pitch:
-            return 'extent'
-    return None
+@pytest.fixture(scope='module')
+def built():
+    import __graft_entry__ as g
+    return g._load_build_module().build()
 
 
 @pytest.mark.parametrize('f8', [False, True])
-def test_fullsize_plan_passes_the_launcher_checks(full, f8):
+def test_fullsize_plan_passes_the_launcher_checks(built, full, f8):
     """The shapes new to the EDM plan path -- 256-wide convolutions as 128-pixel row segments, a 3-channel stem at 256x256,
-    GroupNorm over 65 536-pixel groups, pooling from a 256-wide input, 1024 + 1024 channel concats -- against every launcher check
-    a host can evaluate, at a per-sample-sigma batch of 32 (the affine runs as a GEMM) and at batch 2."""
+    GroupNorm over 65 536-pixel groups, pooling from a 256-wide input, 1024 + 1024 channel concats -- against the launchers' descriptor
+    checks (ds_op_check), at a per-sample-sigma batch of 32 (the affine runs as a GEMM) and at batch 2."""
     _, spec, params = full
     wb, info = planner.pack_weights(spec, params, f8=f8)
     seen = set()
@@ -217,10 +152,10 @@ def test_fullsize_plan_passes_the_launcher_checks(full, f8):
         bad = []
         for i in range(pl.n_ops):
             op = pl.ops_array[i]
-            why = _launcher_guard(op)
-            if why:
-                bad.append((i, S.UNION_FIELD[op.type], why))
             d = getattr(op.u, S.UNION_FIELD[op.type])
+            why = _lib.op_check(d)
+            if why:
+                bad.append((i, why))
             if op.type == S.DS_OP_GEMM and d.a_mode == 0 and d.conv_W == 256:
                 seen.add(('row segment', d.taps, int(d.a_dims[0])))
             if op.type == S.DS_OP_GN_APPLY and d.resample == 1 and d.H == 256:
