@@ -1,5 +1,5 @@
-// Fused softmax attention for sm_90a (head dim padded to 64): O = softmax(scale * Q K^T) V without materialising the L x Lk
-// score matrix in HBM.  Reference: diff-solvers-main/models/networks_edm.py:105-118 (AttentionOp) / :174-178 (UNetBlock attention),
+// Fused softmax attention for sm_90a (head dim padded to 64; 32-wide heads in pairs: attn_pair_kernel): O = softmax(scale * Q K^T) V
+// without materialising the L x Lk score matrix in HBM.  Reference: diff-solvers-main/models/networks_edm.py:105-118 (AttentionOp) / :174-178 (UNetBlock attention),
 // models/ldm/modules/attention.py:152-196 (CrossAttention.forward).
 //
 // One CTA per (sample, head, 128-query tile); keys/values stream through in blocks of 64:
@@ -43,6 +43,7 @@ struct alignas(64) AttnKernelParams {
     long long o_plane;
     int o_pitch;
     int causal;                 // query l sees keys <= l
+    int pair;                   // attn_pair_kernel: 32-wide heads, nh counts head pairs
 };
 
 struct AttnCtl {
@@ -218,11 +219,190 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
     }
 }
 
+// Heads of width 32, two per CTA (ds_attn_desc.pad0 == 32).  The loads are those of attn_kernel with a head PAIR in place of a
+// head: the 64-channel Q / K boxes hold heads 2 hp (channels 0..31) and 2 hp + 1 (32..63) of the pair, the V^T box both heads'
+// 32 d-rows.  Per key block each query warpgroup runs the two heads one after the other:
+//   S_e = Q_e K_e^T   k16 steps 2 e, 2 e + 1 of the swizzled Q / K tiles (3 split-precision passes, as attn_kernel)
+//   online softmax of S_e with its own running max / sum
+//   O_e = alpha_e O_e + P_e V_e   m64n32k16 with B at V^T rows 32 e .. 32 e + 31 (4096 B: whole 1024-byte swizzle atoms)
+// Against 64-wide zero-padded heads this halves the MMAs, the K / V^T bytes and the q/k/v/out GEMM widths.
+__global__ void __launch_bounds__(kAttnThreads, 1) attn_pair_kernel(const __grid_constant__ AttnKernelParams p) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    AttnCtl* ctl = reinterpret_cast<AttnCtl*>(smem + kOffCtl);
+
+    const int wg = threadIdx.x >> 7;
+    const int qt = blockIdx.x % p.q_tiles;
+    const int z = blockIdx.x / p.q_tiles;
+    const int hp = z % p.nh;                        // head pair
+    const int b = z / p.nh;
+    const int lk_eff = p.causal ? min(p.Lk, qt * 128 + 128) : p.Lk;
+    const int nkv = (lk_eff + 63) >> 6;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&p.tmQ);
+        tma_prefetch_desc(&p.tmK);
+        tma_prefetch_desc(&p.tmV);
+        mbar_init(&ctl->q_full, 1);
+        for (int s = 0; s < kAttnStages; ++s) {
+            mbar_init(&ctl->kv_full[s], 1);
+            mbar_init(&ctl->kv_empty[s], 2);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
+            mbar_arrive_expect_tx(&ctl->q_full, kQBytes);
+            tma_load_3d(&p.tmQ, &ctl->q_full, smem, p.q_c0 + hp * 64, qt * 128, b);
+            tma_load_3d(&p.tmQ, &ctl->q_full, smem + 16384, p.q_c0 + hp * 64, qt * 128, p.B + b);
+            for (int j = 0; j < nkv; ++j) {
+                const int s = j % kAttnStages;
+                const uint32_t ph = (j / kAttnStages) & 1;
+                mbar_wait(&ctl->kv_empty[s], ph ^ 1);
+                mbar_arrive_expect_tx(&ctl->kv_full[s], kStageBytes);
+                uint8_t* sk = smem + kOffKV + s * kStageBytes;
+                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk, p.k_c0 + hp * 64, j * 64, b);
+                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk + 8192, p.k_c0 + hp * 64, j * 64, p.B + b);
+                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes, j * 64, hp * 64, b);
+                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes + 8192, j * 64, hp * 64, p.B + b);
+            }
+        }
+        return;
+    }
+
+    const int cw = wg - 1;
+    const int lane = threadIdx.x & 31;
+    const int w = (threadIdx.x >> 5) & 3;
+    const int r0 = cw * 64 + 16 * w + (lane >> 2);
+    const int q0 = qt * 128 + r0;
+    const uint32_t sq = smem_u32(smem) + cw * 64 * 128;
+    float O[2][16];
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) O[e][i] = 0.f;
+    float m[2][2] = {{-INFINITY, -INFINITY}, {-INFINITY, -INFINITY}}, l[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+
+    mbar_wait(&ctl->q_full, 0);
+    for (int j = 0; j < nkv; ++j) {
+        const int s = j % kAttnStages;
+        mbar_wait(&ctl->kv_full[s], (j / kAttnStages) & 1);
+        const uint32_t sk = smem_u32(smem + kOffKV + s * kStageBytes);
+        const uint32_t sv = sk + kKBytes;
+        int kv[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            int lim = p.Lk - j * 64;
+            if (p.causal) lim = min(lim, q0 + 8 * hr - j * 64 + 1);
+            kv[hr] = lim;
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            // Q descriptors are rebuilt per head and block rather than hoisted out of the key loop: kept live, they would be spilled
+            uint32_t sqe = sq;
+            asm volatile("" : "+r"(sqe));
+            float S[32];
+            wgmma_fence();
+#pragma unroll
+            for (int pass = 0; pass < 3; ++pass) {
+                const uint64_t da = wgmma_desc_sw128(sqe + (pass == 1 ? 16384 : 0));
+                const uint64_t db = wgmma_desc_sw128(sk + (pass == 2 ? 8192 : 0));
+#pragma unroll
+                for (int k = 0; k < 2; ++k)
+                    Wgmma<64>::f16(S, da + 2 * (2 * e + k), db + 2 * (2 * e + k), (pass > 0 || k > 0) ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(S);
+
+            float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+                const int hr = (i >> 1) & 1;
+                const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+                if (col < kv[hr]) mx[hr] = fmaxf(mx[hr], S[i]);
+            }
+            float alpha[2], mn[2];
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+                mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+                mn[hr] = fmaxf(m[e][hr], mx[hr] * p.scale_log2e);
+                alpha[hr] = mn[hr] == -INFINITY ? 1.f : ex2_approx(m[e][hr] - mn[hr]);
+            }
+            uint32_t Ph[16], Pl[16];
+            float ls[2] = {0.f, 0.f};
+#pragma unroll
+            for (int i = 0; i < 32; i += 2) {
+                const int hr = (i >> 1) & 1;
+                const int col = 8 * (i >> 2) + 2 * (lane & 3);
+                const float p0 = col < kv[hr] ? ex2_approx(fmaf(S[i], p.scale_log2e, -mn[hr])) : 0.f;
+                const float p1 = col + 1 < kv[hr] ? ex2_approx(fmaf(S[i + 1], p.scale_log2e, -mn[hr])) : 0.f;
+                ls[hr] += p0 + p1;
+                split_h16_pair(p0, p1, Ph[i >> 1], Pl[i >> 1]);
+            }
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                l[e][hr] = l[e][hr] * alpha[hr] + ls[hr];
+                m[e][hr] = mn[hr];
+            }
+            // per-block accumulator folded into O with fp32 FMAs, as in attn_kernel
+            float Ob[16];
+#pragma unroll
+            for (int i = 0; i < 16; ++i) Ob[i] = 0.f;
+            wgmma_fence();
+#pragma unroll
+            for (int pass = 0; pass < 3; ++pass) {
+                const uint32_t* A = pass == 0 ? Pl : Ph;
+                const uint64_t db = wgmma_desc_sw128(sv + e * 4096 + (pass == 1 ? 8192 : 0));
+#pragma unroll
+                for (int kc = 0; kc < 4; ++kc) wgmma_f16_rs_n32(Ob, A + 4 * kc, db + 2 * kc);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(Ob);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) O[e][i] = fmaf(O[e][i], alpha[(i >> 1) & 1], Ob[i]);
+        }
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&ctl->kv_empty[s]);
+    }
+
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            l[e][hr] += __shfl_xor_sync(0xffffffffu, l[e][hr], 1);
+            l[e][hr] += __shfl_xor_sync(0xffffffffu, l[e][hr], 2);
+        }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const int grow = q0 + 8 * hr;
+            if (grow >= p.L) continue;
+            const float inv = 1.f / l[e][hr];
+            __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + hp * 64 + e * 32 + 2 * (lane & 3);
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+                const float v[2] = {O[e][4 * g + 2 * hr] * inv, O[e][4 * g + 2 * hr + 1] * inv};
+                store_planes<2>(o, p.o_plane, 8 * g, v, 2);
+            }
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------ host
+// Width of each head: pad0 of the descriptor (0 = 64).
+static int attn_head_dim(const ds_attn_desc& d) { return d.pad0 == 0 ? 64 : d.pad0; }
+
 OpCheck attn_check(const ds_attn_desc& d) {
     if (d.nplanes != 2 || d.B <= 0 || d.nh <= 0 || d.L <= 0 || d.Lk <= 0 || !(d.scale > 0.f)) return {-30, "attn: args"};
     if (d.q_pitch % 8 || d.k_pitch % 8 || d.vt_pitch % 8 || d.o_pitch % 8 || d.q_c0 % 8 || d.k_c0 % 8) return {-31, "attn: pitch"};
-    if (d.q_c0 + d.nh * 64 > d.q_pitch || d.k_c0 + d.nh * 64 > d.k_pitch || d.nh * 64 > d.o_pitch || d.Lk > d.vt_pitch)
+    const int hd = attn_head_dim(d);
+    if (hd != 64 && hd != 32) return {-41, "attn: head_dim"};
+    // 32-wide heads run in pairs (one 64-channel box): an odd head count is padded with a zero head by the plan
+    if (hd == 32 && d.nh % 2) return {-42, "attn: pair head count"};
+    if (d.q_c0 + d.nh * hd > d.q_pitch || d.k_c0 + d.nh * hd > d.k_pitch || d.nh * hd > d.o_pitch || d.Lk > d.vt_pitch)
         return {-32, "attn: extent"};
     if (d.causal && d.L != d.Lk) return {-40, "attn: causal"};        // the causal mask is defined for self-attention only
     return {0, nullptr};
@@ -243,12 +423,14 @@ int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
         if (encode_map(&kp->tmK, d->k, 3, dims, str, box)) return -34;
     }
     {
-        const int64_t dims[3] = {d->Lk, (int64_t)d->nh * 64, (int64_t)2 * d->B};
-        const int64_t str[2] = {(int64_t)d->vt_pitch * 2, (int64_t)d->nh * 64 * d->vt_pitch * 2};
+        const int64_t rows = (int64_t)d->nh * attn_head_dim(*d);
+        const int64_t dims[3] = {d->Lk, rows, (int64_t)2 * d->B};
+        const int64_t str[2] = {(int64_t)d->vt_pitch * 2, rows * d->vt_pitch * 2};
         const int32_t box[3] = {64, 64, 1};
         if (encode_map(&kp->tmV, d->vt, 3, dims, str, box)) return -35;
     }
-    kp->B = d->B; kp->nh = d->nh; kp->L = d->L; kp->Lk = d->Lk; kp->q_c0 = d->q_c0; kp->k_c0 = d->k_c0;
+    kp->pair = attn_head_dim(*d) == 32 ? 1 : 0;
+    kp->B = d->B; kp->nh = kp->pair ? d->nh / 2 : d->nh; kp->L = d->L; kp->Lk = d->Lk; kp->q_c0 = d->q_c0; kp->k_c0 = d->k_c0;
     kp->q_tiles = (d->L + 127) / 128;
     kp->scale_log2e = d->scale * 1.4426950408889634f;
     kp->out = reinterpret_cast<__half*>(d->out);
@@ -261,17 +443,20 @@ int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
 size_t attn_params_size() { return sizeof(AttnKernelParams); }
 
 int attn_run(const AttnKernelParams* kp, cudaStream_t stream) {
-    static bool attr_set[64] = {};                  // per device (cudaFuncSetAttribute is a per-device setting)
+    static bool attr_set[64][2] = {};               // per device (cudaFuncSetAttribute is a per-device setting) and kernel
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) return -39;
-    if (!attr_set[dev]) {
-        if (cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmem) != cudaSuccess) return -36;
-        attr_set[dev] = true;
+    const int pr = kp->pair ? 1 : 0;
+    if (!attr_set[dev][pr]) {
+        if (cudaFuncSetAttribute(pr ? attn_pair_kernel : attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmem) != cudaSuccess)
+            return -36;
+        attr_set[dev][pr] = true;
     }
     const long long grid = (long long)kp->B * kp->nh * kp->q_tiles;
     if (grid <= 0 || grid > 0x7fffffffLL) return -37;
-    attn_kernel<<<(unsigned)grid, kAttnThreads, kAttnSmem, stream>>>(*kp);
+    if (pr) attn_pair_kernel<<<(unsigned)grid, kAttnThreads, kAttnSmem, stream>>>(*kp);
+    else attn_kernel<<<(unsigned)grid, kAttnThreads, kAttnSmem, stream>>>(*kp);
     return cudaGetLastError() == cudaSuccess ? 0 : -38;
 }
 

@@ -161,7 +161,8 @@ __global__ void __launch_bounds__(1024) gn_finalize_kernel(ds_gn_finalize_desc d
 // ------------------------------------------------------------------------------------------ GN apply
 // grid (chunks, B); block = nc8 * rows threads.  Thread (c8, prow) owns 8 fixed channels: its normalisation coefficients
 // live in registers (mean, a = rstd*gamma*(1+ada_scale), b = beta*(1+ada_scale)+ada_shift) and it streams over output pixels.
-// RESAMPLE 1 (2x2 mean), 2 (nearest x2) or 3 (space-to-depth); resample 0 runs gn_apply_v2_kernel / gn_apply_v3_kernel below.
+// RESAMPLE 1 (2x2 mean), 2 (nearest x2), 3 (space-to-depth) or 4 (space-to-depth at phase pitch pad0); resample 0 runs
+// gn_apply_v2_kernel / gn_apply_v3_kernel below.
 template <int RESAMPLE>
 __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int pix_per_cta, int nc8, int rows) {
     const int C = d.C0 + d.C1;
@@ -191,8 +192,10 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int p
     }
     const int Ho = RESAMPLE == 1 ? d.H / 2 : (RESAMPLE == 2 ? d.H * 2 : d.H);
     const int Wo = RESAMPLE == 1 ? d.W / 2 : (RESAMPLE == 2 ? d.W * 2 : d.W);
-    const int npix = Ho * Wo;              // RESAMPLE == 3 iterates over INPUT pixels and scatters them into the phase layout
-    const long long plane = (long long)d.B * npix * C;
+    const int npix = Ho * Wo;              // RESAMPLE >= 3 iterates over INPUT pixels and scatters them into the phase layout
+    // RESAMPLE == 4: space-to-depth with each phase at a pitch of d.pad0 >= C channels (whole 64-channel GEMM K blocks)
+    const int cp = RESAMPLE == 4 ? d.pad0 : C;
+    const long long plane = (long long)d.B * npix * cp;
     const float* base;
     int pitch, cc;
     if (c < d.C0) { base = d.src0; pitch = d.C0; cc = c; }
@@ -244,13 +247,21 @@ __global__ void __launch_bounds__(512) gn_apply_kernel(ds_gn_apply_desc d, int p
             }
         }
         long long o = ((long long)n * npix + po) * C + c;
-        if (RESAMPLE == 3) {
-            // space-to-depth: input pixel (ho, wo) -> output pixel (ho/2, wo/2), channel block ((ho&1)*2 + (wo&1))*C
+        if (RESAMPLE >= 3) {
+            // space-to-depth: input pixel (ho, wo) -> output pixel (ho/2, wo/2), channel block ((ho&1)*2 + (wo&1))*cp
             const int h2 = ho >> 1, w2 = wo >> 1, ph = ((ho & 1) << 1) | (wo & 1);
-            o = (((long long)n * (d.H / 2) + h2) * (d.W / 2) + w2) * (4LL * C) + (long long)ph * C + c;
+            o = (((long long)n * (d.H / 2) + h2) * (d.W / 2) + w2) * (4LL * cp) + (long long)ph * cp + c;
         }
         if (oact) store_operand<8>(oact, plane, o, act, d.nplanes, d.fmt);
         if (oraw) store_operand<8>(oraw, plane, o, raw, d.nplanes, d.fmt);
+        if (RESAMPLE == 4 && c + 8 == C) {
+            // the phase's channels C .. cp: the GEMM's last K box of the phase reads them, so they must be zero
+            const float zero[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            for (int cz = 8; c + cz < cp; cz += 8) {
+                if (oact) store_operand<8>(oact, plane, o + cz, zero, d.nplanes, d.fmt);
+                if (oraw) store_operand<8>(oraw, plane, o + cz, zero, d.nplanes, d.fmt);
+            }
+        }
         if (d.out_raw_f32) {
             *reinterpret_cast<float4*>(d.out_raw_f32 + o) = make_float4(raw[0], raw[1], raw[2], raw[3]);
             *reinterpret_cast<float4*>(d.out_raw_f32 + o + 4) = make_float4(raw[4], raw[5], raw[6], raw[7]);
@@ -845,6 +856,8 @@ OpCheck dsb::gn_apply_check(const ds_gn_apply_desc& d) {
     if (d.out_act && !d.sums && !d.coef) return {-2, "gn_apply: statistics"};          // a normalised output needs statistics
     // 2x2 pooling and space-to-depth take whole 2x2 blocks: an odd row or column has no output pixel
     if ((d.resample == 1 || d.resample == 3) && (d.H % 2 || d.W % 2)) return {-2, "gn_apply: resample parity"};
+    // pad0: phase pitch of the space-to-depth output (0 = C), a multiple of 8 channels; the f32 raw output has no pitch
+    if (d.pad0 && (d.resample != 3 || d.pad0 < C || d.pad0 % 8 || d.out_raw_f32)) return {-2, "gn_apply: phase pitch"};
     const int nc8 = C / 8;
     if (nc8 > 512) return {-2, "gn_apply: width"};                                   // at most 4096 channels
     // the persistent kernel takes at most 256 threads (2048 channels); wider tensors use the sums path
@@ -891,6 +904,7 @@ extern "C" int ds_gn_apply_launch(const ds_gn_apply_desc* d, cudaStream_t stream
         return ok();
     }
     if (d->resample == 1) gn_apply_kernel<1><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
+    else if (d->resample == 3 && d->pad0 && d->pad0 != C) gn_apply_kernel<4><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
     else if (d->resample == 3) gn_apply_kernel<3><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
     else if (d->resample == 2) gn_apply_kernel<2><<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);
     else gn_apply_v2_kernel<<<grid, threads, 0, stream>>>(*d, pix_per_cta, nc8, rows);

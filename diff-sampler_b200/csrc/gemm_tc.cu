@@ -616,6 +616,8 @@ OpCheck gemm_check(const ds_gemm_desc& d) {
         // e4m3 correction passes: conv mode, one z slice, three passes, a lo plane; the byte planes have no phase channel bases
         if (d.a_mode != 0 || d.num_z != 1 || d.npass != 3 || d.a_plane_n <= 0) return {-16, "gemm: f8"};
         for (int t = 0; t < 9; ++t) if (d.tap_cb[t]) return {-16, "gemm: f8 with tap_cb"};
+        // the e4m3 planes are read in 128-channel boxes whose zero fill the packed weight does not mirror
+        if (d.a_dims[0] % 64 || d.a2_c % 64) return {-16, "gemm: f8 channel remainder"};
     }
     if (d.taps != 1 && d.taps != 9) return {-15, "gemm: taps"};
     // image rows wider than one M tile: the tile is a 128-pixel segment of one row
@@ -640,7 +642,7 @@ int gemm_build(const ds_gemm_desc* d, GemmKernelParams* kp) {
     if (encode_map(&kp->tmB, d->b_ptr, 3, d->b_dims, d->b_strides, bbox)) return -3;
 
     kp->BN = d->BN; kp->m_tiles = d->m_tiles; kp->n_tiles = d->n_tiles; kp->num_z = d->num_z; kp->nh = d->nh > 0 ? d->nh : 1;
-    kp->taps = d->taps; kp->cpb = d->cpb; kp->nkb_main = d->taps * d->cpb; kp->nkb_aux = d->a2_c > 0 ? (int)(d->a2_c / 64) : 0;
+    kp->taps = d->taps; kp->cpb = d->cpb; kp->nkb_main = d->taps * d->cpb; kp->nkb_aux = d->a2_c > 0 ? (int)((d->a2_c + 63) / 64) : 0;
     kp->npass = d->npass; kp->a_mode = d->a_mode; kp->conv_H = d->conv_H; kp->conv_W = d->conv_W;
     kp->a_plane_n = d->a_plane_n; kp->a2_plane_n = d->a2_plane_n; kp->b_plane_batch = d->b_plane_batch;
     kp->a_c_per_zh = d->a_c_per_zh; kp->a_n_per_zb = d->a_n_per_zb; kp->a_n_per_zh = d->a_n_per_zh;

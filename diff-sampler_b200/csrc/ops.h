@@ -139,7 +139,7 @@ typedef struct ds_gn_apply_desc {
     void* out_raw;          // fp16 planes of the raw input; may be NULL
     float* out_raw_f32;     // fp32 raw input at output resolution; may be NULL
     int32_t fmt;            // 0: fp16 hi/lo planes.  1: operand layout of an f8 GEMM (ds_gemm_desc.f8), for out_act and out_raw
-    int32_t pad0;
+    int32_t pad0;           // resample 3: channel pitch of each phase (0 = C); channels C .. pad0 of a phase are written as zeros
     // Precomputed per-(sample, channel) coefficients [B][C][2] = {a, b} with y = x * a + b  (a = rstd * gamma * (1 + ada_scale),
     // b = beta * (1 + ada_scale) + ada_shift - mean * a), written by ds_gn_finalize.  When set (resample == 0 only) the kernel reads
     // them instead of deriving them from `sums` in an fp64 prologue per thread, and runs the persistent, evenly split variant.
@@ -183,7 +183,7 @@ typedef struct ds_attn_desc {
     int32_t nplanes;        // must be 2
     float scale;            // > 0
     int32_t causal;         // 1: query l attends to keys <= l only (CLIP text encoder; L == Lk)
-    int32_t pad0;
+    int32_t pad0;           // head width: 0 or 64, or 32 (heads in pairs: nh even; q/k/out channels and V^T rows at nh*32)
 } ds_attn_desc;
 
 // Row softmax: P = softmax(S) over the last dim, fp32 in, fp16 hi/lo planes out. Reference: networks_edm.py:108.

@@ -83,8 +83,12 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     Output rows are NHWC pixels: out[pixel][cout] (+ fused epilogue).
     edm = (x, coef, coef_stride, C, D): D = c_skip x + c_out y as NCHW fp32 (the EDM combine); nchw_out = (C, D): y as NCHW fp32.
     f8=True: both operands are in the fp16 + 2 x e4m3 layout of csrc/ops.h (activations from ds_gn_apply fmt=1, weights from
-    pack_conv_weight_f8); acc_scale = 2^-S of that packed weight."""
-    assert C % 64 == 0 and C2 % 64 == 0
+    pack_conv_weight_f8); acc_scale = 2^-S of that packed weight.
+    C and C2 need only be multiples of 8: the K loop runs over whole 64-channel blocks, TMA zero-fills the channels past C (C2) in
+    the last block and pack_conv_weight pads each tap (the skip block) to a multiple of 64.  s2d: the space-to-depth input holds
+    each phase at a pitch of C rounded up to 64 channels, the gap zeroed (ds_gn_apply_desc.pad0)."""
+    assert C % 8 == 0 and C2 % 8 == 0
+    cpad, c2pad = -(-C // 64) * 64, -(-C2 // 64) * 64
     if f8:
         assert npass == 3 and not s2d
         a_planes = w_planes = 1          # one fp16 plane; the e4m3 planes sit behind it (the kernel derives their tensor maps)
@@ -94,9 +98,9 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     bw, bh, bnn = conv_box(H, W)
     BN, n_tiles = (bn, -(-Cout // bn)) if bn else fill_bn(Cout, -(-(Bn * H * W) // 128))
     cout_pad = padded_rows(Cout)         # rows of the packed weight; tiles past it read TMA zero fill
-    ktot = taps * C + C2
+    ktot = taps * cpad + c2pad
     d.a_ptr = a_ptr
-    cphys = 4 * C if s2d else C          # physical channel extent of the activation tensor
+    cphys = 4 * cpad if s2d else C       # physical channel extent of the activation tensor
     d.a_dims[:] = [cphys, W, H, a_planes * Bn]
     d.a_strides[:] = [cphys * H16, W * cphys * H16, H * W * cphys * H16]
     d.a_box[:] = [64, bw, bh, bnn]
@@ -104,7 +108,7 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     d.a2_ptr = a2_ptr
     d.a2_c = C2
     d.a2_plane_n = Bn
-    d.nkb_aux = C2 // 64
+    d.nkb_aux = c2pad // 64
     d.b_ptr = w_ptr
     d.b_dims[:] = [ktot, cout_pad, w_planes]
     d.b_strides[:] = [ktot * H16, cout_pad * ktot * H16]
@@ -115,7 +119,7 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
     d.num_z = 1
     d.nh = 1
     d.taps = taps
-    d.cpb = C // 64
+    d.cpb = cpad // 64
     d.npass = npass
     d.a_mode = 0
     d.conv_H, d.conv_W = H, W
@@ -125,7 +129,7 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
             if s2d:     # stride-2 conv over a space-to-depth input: (shift, phase) of input offset kh-1 in {-1, 0, +1}
                 sh, ph = [(-1, 1), (0, 0), (0, 1)][kh]
                 sw, pw = [(-1, 1), (0, 0), (0, 1)][kw]
-                d.tap_dh[t], d.tap_dw[t], d.tap_cb[t] = sh, sw, (ph * 2 + pw) * C
+                d.tap_dh[t], d.tap_dw[t], d.tap_cb[t] = sh, sw, (ph * 2 + pw) * cpad
             else:
                 d.tap_dh[t], d.tap_dw[t], d.tap_cb[t] = kh - 1, kw - 1, 0
     d.m_valid = Bn * H * W

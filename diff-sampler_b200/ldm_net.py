@@ -1,5 +1,6 @@
 """B200LDMNet — native drop-in for the reference's `CFGPrecond` wrapper around a latent-diffusion eps-net
-(networks_edm.py:630-759; Stable Diffusion v1.x `UNetModel`).  Same call contract:
+(networks_edm.py:630-759) around a latent-diffusion eps-net: Stable Diffusion v1.x with classifier-free guidance, or the unconditional
+LSUN-Bedroom / FFHQ LDM-VQ-f4 `UNetModel` (guidance_type='uncond').  Same call contract:
     net(x, sigma, condition=..., unconditional_condition=...) -> D = x - sigma * eps_cfg
 and the attributes the samplers / schedules read (guidance_type, guidance_rate, img_resolution, img_channels, label_dim,
 sigma_min, sigma_max, sigma(), sigma_inv(), round_sigma()).  The eps-net runs in the hand-written kernels (ldm_plan.py);
@@ -23,16 +24,51 @@ def make_alphas_cumprod(linear_start=0.00085, linear_end=0.0120, n=1000):
     return torch.cumprod(1.0 - betas, dim=0).to(torch.float32)
 
 
+UNCOND_BETAS = (0.0015, 0.0195)       # linear_start / linear_end of lsun_bedrooms-ldm-vq-4.yaml and ffhq-ldm-vq-4.yaml
+
+
+def load_ldm_checkpoint(path):
+    """The released LDM `model.ckpt` (a LatentDiffusion state dict under 'state_dict') read with torch.load(weights_only=True), never
+    unpickled further -> (eps-net state dict (`model.diffusion_model.*`), VQ first-stage decoder state dict (`first_stage_model.`
+    decoder / post_quant_conv / codebook), alphas_cumprod or None, scale_factor)."""
+    import pickle
+    try:
+        ck = torch.load(path, map_location='cpu', weights_only=True)
+    except pickle.UnpicklingError as e:
+        raise ValueError(f'{path}: not loadable with torch.load(weights_only=True); it is not unpickled any further, since a full '
+                         f'unpickle can run arbitrary code.  Re-save its state_dict alone to use it here.  ({e})') from None
+    if not isinstance(ck, dict) or not isinstance(ck.get('state_dict'), dict):
+        raise ValueError(f'{path}: no state_dict in the checkpoint')
+    sd = ck['state_dict']
+    unet = OrderedDict((k[len('model.diffusion_model.'):], v) for k, v in sd.items() if k.startswith('model.diffusion_model.'))
+    first = OrderedDict((k[len('first_stage_model.'):], v) for k, v in sd.items() if k.startswith('first_stage_model.')
+                        and k[len('first_stage_model.'):].startswith(('decoder.', 'post_quant_conv.', 'quantize.embedding.')))
+    if not unet or not first:
+        raise ValueError(f'{path}: expected model.diffusion_model.* and first_stage_model.* keys of a LatentDiffusion checkpoint')
+    sf = sd.get('scale_factor')
+    return unet, first, sd.get('alphas_cumprod'), float(sf) if sf is not None else 1.0
+
+
 class B200LDMNet:
     def __init__(self, params, img_resolution=64, img_channels=4, num_heads=8, alphas_cumprod=None, guidance_type='classifier-free',
-                 guidance_rate=1.0, epsilon_t=1e-3, precision=None, device='cuda', flash_attn=True, f8_linear=None, cuda_graph=None):
+                 guidance_rate=1.0, epsilon_t=1e-3, precision=None, device='cuda', flash_attn=True, f8_linear=None, cuda_graph=None,
+                 num_head_channels=-1, head_pairs=True):
+        """guidance_type 'uncond': the unconditional nets (no context, one pass per call); their legacy attention layers take
+        num_head_channels (32 for LDM-VQ-f4) and, with head_pairs, run their 32-wide heads two per CTA."""
+        if guidance_type not in ('classifier-free', 'uncond'):
+            raise ValueError(f'B200LDMNet: guidance_type {guidance_type!r} is not one of classifier-free, uncond')
         self.device = torch.device(device)
         if self.device.type != 'cuda':
             raise _lib.DsError('B200LDMNet needs a CUDA device (no CPU fallback)')
-        self.lib = _lib.load()
-        self.img_resolution, self.img_channels, self.label_dim = img_resolution, img_channels, True
-        self.guidance_type, self.guidance_rate = guidance_type, guidance_rate
+        self.uncond = guidance_type == 'uncond'
         self.precision = precision or default_precision()
+        if self.uncond and self.precision == 'fp16f8':
+            raise ValueError('B200LDMNet: fp16f8 is not available for the unconditional nets: the f8 GEMM mode needs channel counts that '
+                             'are multiples of 64, and their 224 / 672 / 1120 / 1568-channel convolutions are not')
+        self.lib = _lib.load()
+        self.img_resolution, self.img_channels = img_resolution, img_channels
+        self.label_dim = 0 if self.uncond else True
+        self.guidance_type, self.guidance_rate = guidance_type, guidance_rate
         self.npass = PRECISIONS[self.precision]
         self.f8 = self.precision == 'fp16f8'           # ResBlock convolutions in the f8 GEMM mode (csrc/ops.h)
         # with fp16f8, proj_in / attn2.to_q / GEGLU ff / proj_out also run in the f8 GEMM mode (held by the f8 parity tests;
@@ -43,11 +79,16 @@ class B200LDMNet:
         self.f8_linear = bool(f8_linear) and self.f8
         self.flash_attn = bool(flash_attn)
         self.cuda_graph = default_cuda_graph() if cuda_graph is None else bool(cuda_graph)
-        self.st = ldm_plan.ldm_structure(params, num_heads)
-        self.wb, self.info = ldm_plan.pack_ldm_weights(self.st, params, f8=self.f8, f8_linear=self.f8_linear)
+        self.st = ldm_plan.ldm_structure(params, num_heads, num_head_channels)
+        self.wb, self.info = ldm_plan.pack_ldm_weights(self.st, params, f8=self.f8, f8_linear=self.f8_linear, head_pairs=head_pairs)
+        if self.uncond and self.info['ctx_dim'] is not None:
+            raise ValueError('B200LDMNet: guidance_type uncond given for a net with cross-attention')
         self.native = _lib.NativePlans(self.wb.bytes(), self.device)
         self.total_launches = 0
-        ac = make_alphas_cumprod() if alphas_cumprod is None else torch.as_tensor(alphas_cumprod).float()
+        if alphas_cumprod is None:
+            ac = make_alphas_cumprod(*UNCOND_BETAS) if self.uncond else make_alphas_cumprod()
+        else:
+            ac = torch.as_tensor(alphas_cumprod).detach().float().cpu()
         log_alphas = 0.5 * torch.log(ac)
         self.M = len(log_alphas)
         self.t_array = torch.linspace(0., 1., self.M + 1)[1:].reshape((1, -1))
@@ -63,8 +104,20 @@ class B200LDMNet:
         nh = getattr(unet, 'num_heads', num_heads)          # openaimodel.py:466 (-1 when the config gives num_head_channels instead)
         if isinstance(nh, int) and nh > 0:
             num_heads = nh
+        nhc = getattr(unet, 'num_head_channels', -1)
         return cls(sd, img_resolution=net.img_resolution, img_channels=net.img_channels, num_heads=num_heads,
-                   alphas_cumprod=net.model.alphas_cumprod, guidance_type=net.guidance_type, guidance_rate=net.guidance_rate, **kw)
+                   alphas_cumprod=net.model.alphas_cumprod, guidance_type=net.guidance_type, guidance_rate=net.guidance_rate,
+                   num_head_channels=nhc if isinstance(nhc, int) else -1, **kw)
+
+    @classmethod
+    def from_ldm_checkpoint(cls, path, img_resolution=64, num_head_channels=32, device='cuda', **kw):
+        """The unconditional LSUN-Bedroom / FFHQ LDM-VQ-f4 `model.ckpt` -> (eps-net as B200LDMNet(guidance_type='uncond'), its VQ
+        decoder as B200VAEDecoder).  The file is read with torch.load(weights_only=True) only (load_ldm_checkpoint)."""
+        from .vae_net import B200VAEDecoder
+        unet, first, ac, sf = load_ldm_checkpoint(path)
+        net = cls(unet, img_resolution=img_resolution, img_channels=unet['input_blocks.0.0.weight'].shape[1], guidance_type='uncond',
+                  num_head_channels=num_head_channels, alphas_cumprod=ac, device=device, **kw)
+        return net, B200VAEDecoder(first, scale_factor=sf, device=device)
 
     # ---- VP <-> sigma mapping (networks_edm.py:694-718; piecewise-linear interpolation :720-756) ---------------------------------
     @staticmethod
@@ -100,20 +153,23 @@ class B200LDMNet:
     # ---- plan cache ---------------------------------------------------------------------------------------------------------
     def _plan(self, B, Bt, nT):
         px = self.img_channels * self.img_resolution ** 2 * 4
+        ctx_f = self.info['ctx_dim'] or 0
         return self.native.get((B, Bt, nT),
                                lambda: ldm_plan.compile_ldm_plan(self.st, self.wb, self.info, B, Bt, nT, self.img_resolution, npass=self.npass,
                                                                  flash_attn=self.flash_attn, f8=self.f8, f8_linear=self.f8_linear),
                                (lambda pl: (B * px, Bt * px, nT * 4, (B if nT > 1 else 1) * 16, Bt * 64 * 4,
-                                            Bt * pl.meta['ctx_tokens'] * self.info['ctx_dim'] * 4)) if self.cuda_graph else None)
+                                            Bt * pl.meta['ctx_tokens'] * ctx_f * 4)) if self.cuda_graph else None)
 
     def eps(self, x_scaled_src, coef, tvals, context, bottleneck=None):
-        """eps-net on Bt = context.shape[0] samples: inputs x [B,...] (c_in applied in-kernel via coef[:,2]), timesteps tvals [1|Bt]."""
-        B, Bt = x_scaled_src.shape[0], context.shape[0]
+        """eps-net on Bt = context.shape[0] samples (B without context): inputs x [B,...] (c_in applied in-kernel via coef[:,2]),
+        timesteps tvals [1|Bt]."""
+        B = x_scaled_src.shape[0]
+        Bt = context.shape[0] if context is not None else B
         nT = tvals.numel()
         h, pl = self._plan(B, Bt, nT)
         out = torch.empty((Bt,) + tuple(x_scaled_src.shape[1:]), device=x_scaled_src.device)
         io = (x_scaled_src.data_ptr(), out.data_ptr(), tvals.data_ptr(), coef.data_ptr(), bottleneck.data_ptr() if bottleneck is not None else None,
-              context.data_ptr())
+              context.data_ptr() if context is not None else None)
         self.total_launches += self.native.run(h, io, torch.cuda.current_stream(x_scaled_src.device).cuda_stream)
         return out
 
@@ -129,9 +185,9 @@ class B200LDMNet:
         coef = torch.zeros(sig.numel(), 4, device=x.device)
         coef[:, 2] = c_in
         cfg = self.guidance_type == 'classifier-free' and not (self.guidance_rate == 1. or unconditional_condition is None)
-        if self.guidance_type == 'uncond':
-            raise NotImplementedError('unconditional latent-diffusion nets are not lowered (no context)')
-        if cfg:
+        if self.uncond:
+            ctx, tvals = None, c_noise
+        elif cfg:
             ctx = torch.cat([unconditional_condition, condition]).to(torch.float32).contiguous()
             tvals = c_noise if c_noise.numel() == 1 else torch.cat([c_noise] * 2)
         else:
@@ -140,10 +196,10 @@ class B200LDMNet:
         tvals = tvals.contiguous()
         bott = None
         if bottleneck is not None:
-            bott = torch.empty(ctx.shape[0], 64, device=x.device)
+            bott = torch.empty(ctx.shape[0] if ctx is not None else B, 64, device=x.device)
         F = self.eps(x, coef.contiguous(), tvals, ctx, bottleneck=bott)
         if bottleneck is not None:
-            bottleneck.copy_(bott[-B:])           # the conditional half (solvers_amed.py:24-25)
+            bottleneck.copy_(bott[-B:])           # the conditional half (solvers_amed.py:24-25), or the whole batch (uncond)
         if out is None:
             out = torch.empty_like(x)
         # D = x - sigma * (eps_u + g (eps_c - eps_u))   [c_skip = 1, c_out = -sigma]; one fused update kernel

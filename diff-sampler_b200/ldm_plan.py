@@ -5,6 +5,11 @@ Downsample :134-160, Upsample :91-119; models/ldm/modules/attention.py SpatialTr
 CrossAttention :170-193, GEGLU :42-44; util.py:151-171 (timestep_embedding).  Same op set and executor as the EDM nets (plan.py):
 every contraction is the wgmma GEMM kernel; LayerNorm / GEGLU / softmax / GroupNorm are the HBM-bound companions.
 
+The unconditional LSUN-Bedroom / FFHQ LDM-VQ-f4 eps-nets (models/ldm/configs/latent-diffusion/lsun_bedrooms-ldm-vq-4.yaml) use the
+same UNetModel with the legacy AttentionBlock (openaimodel.py:278-324, QKVAttentionLegacy :347-372) instead of the SpatialTransformer:
+GroupNorm -> qkv 1x1 -> softmax attention over 32-wide heads -> proj_out -> residual, and have no cross-attention.  Their level widths
+(224, 672) and concat widths (1568, 1120) are not multiples of 64: the GEMMs zero-fill the last 64-channel K block (gemm_desc.conv_gemm).
+
 Layout notes specific to this net:
   * head dims 40 / 80 / 160 are zero-padded to 64 / 128 / 192 inside the packed q/k/v/out weights (K blocks are 64 wide);
   * the 77 context tokens are not padded in memory: K extents / key counts that are not multiples of 64 are zero-filled by TMA;
@@ -28,9 +33,10 @@ def dpad(d):
     return -(-d // 64) * 64
 
 
-def ldm_structure(params, num_heads):
+def ldm_structure(params, num_heads, num_head_channels=-1):
     """Block structure from UNetModel.state_dict() names/shapes:
-    [(block_name, [('conv'|'res'|'attn'|'down'|'up', module_name, ...)])] for input / middle / output blocks."""
+    [(block_name, [('conv'|'res'|'attn'|'qkv_attn'|'down'|'up', module_name, ...)])] for input / middle / output blocks.
+    Heads per attention layer: ch // num_head_channels when num_head_channels > 0 (openaimodel.py:540-544), else num_heads."""
     names = list(params.keys())
     mods = OrderedDict()
     for k in names:
@@ -46,6 +52,10 @@ def ldm_structure(params, num_heads):
             ch = params[mod + '.norm.weight'].shape[0]
             inner = params[mod + '.proj_in.weight'].shape[0]
             return ('attn', mod, ch, num_heads, inner // num_heads)
+        if (mod + '.qkv.weight') in params:           # legacy AttentionBlock
+            ch = params[mod + '.norm.weight'].shape[0]
+            heads = ch // num_head_channels if num_head_channels > 0 else num_heads
+            return ('qkv_attn', mod, ch, heads, ch // heads)
         if (mod + '.op.weight') in params:
             w = params[mod + '.op.weight']
             return ('down', mod, w.shape[1], w.shape[0])
@@ -86,14 +96,46 @@ def _pad_heads_cols(w, heads, dh):
     return out
 
 
-def pack_ldm_weights(st, params, f8=False, f8_linear=False):
+def _legacy_qkv_split(w, b, heads, pairs):
+    """The legacy AttentionBlock's qkv rows, ordered [head][q|k|v][d] (QKVAttentionLegacy, openaimodel.py:361-363), as
+    [q heads | k heads] rows and separate v rows, each head in a slot of 32 rows (pairs: the head count rounded up to even, the extra
+    head all zeros) or of 64 rows (the zero-padded layout of the 64-wide attention kernel).  Returns (w_qk, b_qk, w_v, b_v)."""
+    c3 = w.shape[0]
+    d = c3 // 3 // heads
+    dp = 32 if pairs else dpad(d)
+    hs = heads + heads % 2 if pairs else heads
+    w3 = w.reshape(heads, 3, d, -1)
+    b3 = b.reshape(heads, 3, d)
+
+    def slots(x):
+        out = torch.zeros((hs, dp) + tuple(x.shape[2:]), dtype=x.dtype)
+        out[:heads, :d] = x
+        return out.reshape((hs * dp,) + tuple(x.shape[2:]))
+    wq, wk, wv = (slots(w3[:, i]) for i in range(3))
+    bq, bk, bv = (slots(b3[:, i]) for i in range(3))
+    return torch.cat([wq, wk]), torch.cat([bq, bk]), wv, bv
+
+
+def _legacy_proj_cols(w, heads, pairs):
+    """proj_out weight [C, heads*d] -> [C, slots*dp]: zero columns for the padding rows / head of _legacy_qkv_split."""
+    d = w.shape[1] // heads
+    dp = 32 if pairs else dpad(d)
+    hs = heads + heads % 2 if pairs else heads
+    out = torch.zeros(w.shape[0], hs, dp, dtype=w.dtype)
+    out[:, :heads, :d] = w.reshape(w.shape[0], heads, d)
+    return out.reshape(w.shape[0], hs * dp)
+
+
+def pack_ldm_weights(st, params, f8=False, f8_linear=False, head_pairs=True):
     """f8=True: the ResBlock convolutions (in_layers.2, out_layers.3 + skip_connection) are packed for the f8 GEMM mode (csrc/ops.h).
     f8_linear=True (opt-in, needs f8): also the transformer linears whose A operand has a single consumer -- proj_in, attn2.to_q, the
-    GEGLU feed-forward pair and proj_out (75 % of the transformer's linear FLOPs)."""
+    GEGLU feed-forward pair and proj_out (75 % of the transformer's linear FLOPs).
+    head_pairs: the legacy attention's 32-wide heads run two per CTA (attn_pair_kernel); False pads each head to 64 (attn_kernel),
+    kept as a comparator."""
     assert f8 or not f8_linear
     P = lambda k: params[k].detach().float().cpu()
     wb = WeightBlob()
-    info = dict(res=[], ctx_dim=None, f8_shift={})
+    info = dict(res=[], ctx_dim=None, f8_shift={}, head_pairs=bool(head_pairs))
 
     def add_conv(key, w, skip_w=None, bias=None, as_f8=False):
         shift = wb.add_gemm(key, w, skip_w, bias, f8=as_f8)[1]
@@ -145,6 +187,15 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False):
                 add_conv(t + '.ff1', P(t + '.ff.net.0.proj.weight'), bias=P(t + '.ff.net.0.proj.bias'), as_f8=f8_linear)
                 add_conv(t + '.ff2', P(t + '.ff.net.2.weight'), bias=P(t + '.ff.net.2.bias'), as_f8=f8_linear)
                 add_conv(n + '.proj_out', P(n + '.proj_out.weight').reshape(ch, heads * dh), bias=P(n + '.proj_out.bias'), as_f8=f8_linear)
+            elif kind == 'qkv_attn':
+                _, _, ch, heads, dh = L
+                wb.add_norm(n + '.norm', P)
+                wqk, bqk, wv, bv = _legacy_qkv_split(P(n + '.qkv.weight').reshape(3 * ch, ch), P(n + '.qkv.bias'), heads, head_pairs)
+                add_conv(n + '.qk', wqk, bias=bqk)
+                wb.add(n + '.v:w', G.split_planes(wv))
+                wb.add(n + '.v:b', bv)
+                add_conv(n + '.proj_out', _legacy_proj_cols(P(n + '.proj_out.weight').reshape(ch, ch), heads, head_pairs),
+                         bias=P(n + '.proj_out.bias'))
             elif kind == 'down':
                 add_conv(n, P(n + '.op.weight'), bias=P(n + '.op.bias'))
             elif kind == 'up':
@@ -160,7 +211,8 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False):
 def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_attn=True, f8=False, f8_linear=False):
     """Lower the eps-net for Bt samples (Bt = B, or 2B under classifier-free guidance) at latent resolution R.
     nT in {1, Bt}: number of timestep values.  io: X = x [B,C,R,R], SIGMA = timesteps [nT], LABELS = coef [B|1][4] (c_in in slot 2),
-    CTX = context [Bt, 77, ctx_dim], D = eps [Bt,C,R,R] (NCHW), BOTTLENECK = channel-mean of the middle block [Bt, 64]."""
+    CTX = context [Bt, 77, ctx_dim] (nets with cross-attention only), D = eps [Bt,C,R,R] (NCHW), BOTTLENECK = channel-mean of the
+    middle block [Bt, 64]."""
     assert nT in (1, Bt)
     assert not f8 or (npass == 3 and info['f8_shift'])
     assert f8 or not f8_linear
@@ -175,7 +227,8 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
     cd = info['ctx_dim']
     T = ctx_tokens
     TP = CTX_TOKENS_PITCH
-    pb.stats(sum(2 if L[0] == 'res' else (1 if L[0] == 'attn' else 0) for _, ls in st['inp'] + st['mid'] + st['out'] for L in ls) + 1)
+    pb.stats(sum(2 if L[0] == 'res' else (1 if L[0] in ('attn', 'qkv_attn') else 0) for _, ls in st['inp'] + st['mid'] + st['out'] for L in ls)
+             + 1)
     # ---------------- timestep embedding (util.py:151-171, openaimodel.py:723-724) + all emb_layers in one launch -------------
     pb.need('emb0', nT * mc * F4)
     pb.need('e1', nT * ted * F4)
@@ -193,8 +246,9 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
     aff_stride = info['aff_total'] if nT > 1 else 0
     aff_off = dict(info['res'])
     # ---------------- context tokens -> fp16 planes (once per forward, shared by every cross-attention) ------------------------
-    pb.need('ctx', NPL * Bt * T * cd * H2)
-    pb.to_planes(io(S.DS_IO_CTX), cd, T, 1, Bt, 'ctx')
+    if cd is not None:
+        pb.need('ctx', NPL * Bt * T * cd * H2)
+        pb.to_planes(io(S.DS_IO_CTX), cd, T, 1, Bt, 'ctx')
 
     def lower_res(L, parts, H):
         """ResBlock (openaimodel.py:255-275): GN+SiLU+conv3x3, + Linear(SiLU(emb)), GN+SiLU+conv3x3, + skip (identity | 1x1)."""
@@ -278,11 +332,34 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
                                     bias=W(n + '.proj_out:b'), residual=R_(src), ldr=ch, **f8_args(n + '.proj_out'))[0])
         return out, ch
 
+    def lower_qkv_attn(L, src, H):
+        """Legacy AttentionBlock (openaimodel.py:310-324): x + proj_out(attention(qkv(GroupNorm(x)))), softmax scale 1/sqrt(d)."""
+        _, n, ch, heads, dh = L
+        pairs = info['head_pairs']
+        hs, dp = (heads + heads % 2, 32) if pairs else (heads, dpad(dh))
+        hp = hs * dp
+        Lq = H * H
+        M = Bt * Lq
+        pb.need('act', NPL * M * ch * H2)
+        pb.group_norm([(src, ch)], H, n + '.norm', 1e-5, 'act', silu=0)
+        pb.need('qk', NPL * M * 2 * hp * H2)
+        pb.need('vt', NPL * Bt * hp * Lq * H2)
+        pb.need('o', NPL * M * hp * H2)
+        emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, ch, W(n + '.qk:w'), 2 * hp, taps=1, npass=npass, out_h16=R_('qk'),
+                                    bias=W(n + '.qk:b'))[0])
+        pb.vt_gemm(n + '.v:w', 'act', ch, hp, Lq, Lq, bias=n + '.v:b')
+        pb.attention(flash_attn or pairs, 'qk', 'qk', 'o', hs, Lq, Lq, dp, dh ** -0.5, Lq, pairs=pairs)
+        out = pb.need('h:' + n, M * ch * F4)
+        emit(lambda R_: G.conv_gemm(R_('o'), Bt, H, H, hp, W(n + '.proj_out:w'), ch, taps=1, npass=npass, out_f32=R_(out),
+                                    bias=W(n + '.proj_out:b'), residual=R_(src), ldr=ch)[0])
+        return out, ch
+
     def lower_down(L, src, H):
         _, n, cin, cout = L
         Ho = H // 2
-        pb.need('s2d', NPL * Bt * H * H * cin * H2)
-        pb.to_planes(src, cin, H, H, Bt, 's2d', resample=3)
+        cpad = dpad(cin)            # each space-to-depth phase starts on a 64-channel K block of the GEMM
+        pb.need('s2d', NPL * Bt * H * H * cpad * H2)
+        pb.to_planes(src, cin, H, H, Bt, 's2d', resample=3, phase_pitch=cpad if cpad != cin else 0)
         out = pb.need('h:' + n, Bt * Ho * Ho * cout * F4)
         emit(lambda R_: G.conv_gemm(R_('s2d'), Bt, Ho, Ho, cin, W(n + ':w'), cout, taps=9, npass=npass, out_f32=R_(out), bias=W(n + ':b'),
                                     s2d=True)[0])
@@ -316,6 +393,8 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
                 cur, cur_c = lower_res(L, [(cur, cur_c)], H)
             elif L[0] == 'attn':
                 cur, cur_c = lower_attn(L, cur, H)
+            elif L[0] == 'qkv_attn':
+                cur, cur_c = lower_qkv_attn(L, cur, H)
             elif L[0] == 'down':
                 cur, cur_c, H = lower_down(L, cur, H)
         hs.append((cur, cur_c))
@@ -323,6 +402,8 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
         pb.tag += 1
         if L[0] == 'res':
             cur, cur_c = lower_res(L, [(cur, cur_c)], H)
+        elif L[0] == 'qkv_attn':
+            cur, cur_c = lower_qkv_attn(L, cur, H)
         else:
             cur, cur_c = lower_attn(L, cur, H)
     mid_out, mid_c, mid_H = cur, cur_c, H
@@ -337,6 +418,8 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
                 cur, cur_c = lower_res(L, parts, H)
             elif L[0] == 'attn':
                 cur, cur_c = lower_attn(L, cur, H)
+            elif L[0] == 'qkv_attn':
+                cur, cur_c = lower_qkv_attn(L, cur, H)
             elif L[0] == 'up':
                 cur, cur_c, H = lower_up(L, cur, H)
             first_layer = False

@@ -153,11 +153,12 @@ class PlanBuilder:
                                           sums=R('stats', slot)))
 
     def gn_apply(self, parts, H, norm, eps, out, *, W=None, B=None, groups=32, slot=None, coef=False, silu=1, ada=None, ada_stride=0,
-                 resample=0, raw=None, raw_f32=None, fmt=0):
+                 resample=0, raw=None, raw_f32=None, fmt=0, phase_pitch=0):
         """GroupNorm of `parts` (as gn_stats; an input may also be an io reference) with the gain / bias `norm`:g / `norm`:b (+ SiLU)
         into the activation operand `out`: fp16 planes, or the f8 operand image (fmt=1).  The statistics are the sums of stats slot
         `slot`, or the coefficient table 'gncoef' (coef=True).  raw / raw_f32 also receive the input un-normalised (fp16 planes /
-        fp32); resample 1 / 2 / 3 = 2x2 average pooling / nearest x2 / space-to-depth.  norm=None: no normalisation."""
+        fp32); resample 1 / 2 / 3 = 2x2 average pooling / nearest x2 / space-to-depth (phase_pitch: channels per phase, 0 = C).
+        norm=None: no normalisation."""
         (n0, c0), (n1, c1) = parts[0], (parts[1] if len(parts) > 1 else (None, 0))
         assert norm is None or (c0 + c1) % groups == 0
         Wt = self.wb.ref
@@ -166,7 +167,7 @@ class PlanBuilder:
             sums=R('stats', slot) if slot is not None and not coef else 0, coef=R('gncoef') if coef else 0,
             gamma=Wt(norm + ':g') if norm else 0, beta=Wt(norm + ':b') if norm else 0, eps=eps, silu=silu,
             ada=_resolve(R, ada), ada_stride=ada_stride, resample=resample, nplanes=NPL, out_act=_resolve(R, out),
-            out_raw=_resolve(R, raw), out_raw_f32=_resolve(R, raw_f32), fmt=fmt))
+            out_raw=_resolve(R, raw), out_raw_f32=_resolve(R, raw_f32), fmt=fmt, pad0=phase_pitch))
 
     def group_norm(self, parts, H, norm, eps, out, **apply_kw):
         """GroupNorm from sums: a statistics pass into a fresh stats slot, then gn_apply."""
@@ -174,29 +175,33 @@ class PlanBuilder:
         self.gn_stats(slot, parts, H * H)
         self.gn_apply(parts, H, norm, eps, out, slot=slot, **apply_kw)
 
-    def to_planes(self, src, C, H, W, B, dst, fmt=0, resample=0, groups=32):
+    def to_planes(self, src, C, H, W, B, dst, fmt=0, resample=0, groups=32, phase_pitch=0):
         """fp32 NHWC -> the fp16 hi/lo planes (or, fmt=1, the f8 operand image) of a GEMM operand, without normalisation."""
-        self.gn_apply([(src, C)], H, None, 0.0, None, W=W, B=B, groups=groups, silu=0, resample=resample, raw=dst, fmt=fmt)
+        self.gn_apply([(src, C)], H, None, 0.0, None, W=W, B=B, groups=groups, silu=0, resample=resample, raw=dst, fmt=fmt,
+                      phase_pitch=phase_pitch)
 
     # ---- attention --------------------------------------------------------------------------------------------------------------
     def vt_gemm(self, w, src, C, N, L, pitch, bias=None):
         """V^T[b][n][key] = sum_c Wv[n][c] src[b][key][c] (+ bias[n]) into 'vt' (rows of `pitch` keys), the layout the P.V product
-        reads: the weight's fp16 planes `w` [2][N][C] are the M operand, the B batch entries' L rows of `src` the N operand."""
+        reads: the weight's fp16 planes `w` [2][N][C] are the M operand, the B batch entries' L rows of `src` the N operand.  C % 64 != 0:
+        the K loop runs to C rounded up to 64, both operands' last block zero-filled by TMA."""
         W = self.wb.ref
-        self.emit(lambda R: G.rows_gemm(W(w), N, C, 1, R(src), L, C, self.B, C, num_z=self.B, nh=1, m_valid=N, n_valid=L,
+        K = -(-C // 64) * 64
+        self.emit(lambda R: G.rows_gemm(W(w), N, C, 1, R(src), L, C, self.B, K, num_z=self.B, nh=1, m_valid=N, n_valid=L,
                                         npass=self.npass, b_z_per_zb=1, out_h16=R('vt'), o_zb=N * pitch, ldo=pitch,
                                         o_plane=self.B * N * pitch, bias_m=W(bias) if bias else 0)[0])
 
-    def attention(self, fused, q, k, out, nh, L, Lk, d, scale, vt_pitch, causal=0, s_pitch=None):
+    def attention(self, fused, q, k, out, nh, L, Lk, d, scale, vt_pitch, causal=0, s_pitch=None, pairs=False):
         """softmax(scale Q K^T) V for nh heads of width d over the B batch entries: L queries, Lk keys, V^T in 'vt' (rows of vt_pitch
         keys), O into the fp16 planes `out` [B][L][nh d].  q == k: one [q heads | k heads] buffer of pitch 2 nh d, else two of nh d.
-        fused: the fused kernel (csrc/attention.cu, 64-wide heads); otherwise QK^T into 'S' (rows of s_pitch, default Lk), the row
+        fused: the fused kernel (csrc/attention.cu, 64-wide heads, or pairs=True: 32-wide heads two per CTA, nh even); otherwise QK^T into 'S' (rows of s_pitch, default Lk), the row
         softmax into 'P' (rows of vt_pitch) and the P.V GEMM."""
         B, C = self.B, nh * d
         qp, kc0 = (2 * C, C) if q == k else (C, 0)
         if fused:
             self.emit(lambda R: S.AttnDesc(q=R(q), k=R(k), vt=R('vt'), out=R(out), B=B, nh=nh, L=L, Lk=Lk, q_pitch=qp, q_c0=0,
-                                           k_pitch=qp, k_c0=kc0, vt_pitch=vt_pitch, o_pitch=C, nplanes=NPL, scale=scale, causal=causal))
+                                           k_pitch=qp, k_c0=kc0, vt_pitch=vt_pitch, o_pitch=C, nplanes=NPL, scale=scale, causal=causal,
+                                           pad0=32 if pairs else 0))
             return
         sp = s_pitch or Lk
         self.need('S', B * nh * L * sp * F4)
