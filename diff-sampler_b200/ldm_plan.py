@@ -131,17 +131,11 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False, head_pairs=True):
     f8_linear=True (opt-in, needs f8): also the transformer linears whose A operand has a single consumer -- proj_in, attn2.to_q, the
     GEGLU feed-forward pair and proj_out (75 % of the transformer's linear FLOPs).
     head_pairs: the legacy attention's 32-wide heads run two per CTA (attn_pair_kernel); False pads each head to 64 (attn_kernel),
-    kept as a comparator."""
+    kept as a comparator.  info['f8_shift'] is the blob's own record of the f8-packed GEMMs (WeightBlob.f8_shift)."""
     assert f8 or not f8_linear
     P = lambda k: params[k].detach().float().cpu()
     wb = WeightBlob()
-    info = dict(res=[], ctx_dim=None, f8_shift={}, head_pairs=bool(head_pairs))
-
-    def add_conv(key, w, skip_w=None, bias=None, as_f8=False):
-        shift = wb.add_gemm(key, w, skip_w, bias, f8=as_f8)[1]
-        if as_f8:
-            info['f8_shift'][key] = shift
-
+    info = dict(res=[], ctx_dim=None, head_pairs=bool(head_pairs), f8_shift=wb.f8_shift)
     for k in ('time_embed.0', 'time_embed.2'):
         wb.add(k + ':w', P(k + '.weight'))
         wb.add(k + ':b', P(k + '.bias'))
@@ -151,17 +145,10 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False, head_pairs=True):
         for L in layers:
             kind, n = L[0], L[1]
             if kind == 'conv':
-                add_conv(n, P(n + '.weight'), bias=P(n + '.bias'))
+                wb.add_gemm(n, P(n + '.weight'), bias=P(n + '.bias'))
             elif kind == 'res':
-                wb.add_norm(n + '.n0', P, n + '.in_layers.0')
-                add_conv(n + '.c0', P(n + '.in_layers.2.weight'), bias=P(n + '.in_layers.2.bias'), as_f8=f8)
-                wb.add_norm(n + '.n1', P, n + '.out_layers.0')
-                b1 = P(n + '.out_layers.3.bias')
-                skw = None
-                if (n + '.skip_connection.weight') in params:
-                    skw = P(n + '.skip_connection.weight')
-                    b1 = b1 + P(n + '.skip_connection.bias')
-                add_conv(n + '.c1', P(n + '.out_layers.3.weight'), skw, bias=b1, as_f8=f8)
+                skip = n + '.skip_connection' if (n + '.skip_connection.weight') in params else None
+                wb.add_res_block(n, P, n + '.in_layers.0', n + '.in_layers.2', n + '.out_layers.0', n + '.out_layers.3', skip, f8=f8)
                 aff_w.append(P(n + '.emb_layers.1.weight'))
                 aff_b.append(P(n + '.emb_layers.1.bias'))
                 info['res'].append((n, aff_off))
@@ -170,41 +157,37 @@ def pack_ldm_weights(st, params, f8=False, f8_linear=False, head_pairs=True):
                 _, _, ch, heads, dh = L
                 t = n + '.transformer_blocks.0'
                 wb.add_norm(n + '.norm', P)
-                add_conv(n + '.proj_in', P(n + '.proj_in.weight').reshape(heads * dh, ch), bias=P(n + '.proj_in.bias'), as_f8=f8_linear)
+                wb.add_gemm(n + '.proj_in', P(n + '.proj_in.weight').reshape(heads * dh, ch), bias=P(n + '.proj_in.bias'), f8=f8_linear)
                 for k in (1, 2, 3):
                     wb.add_norm(f'{t}.norm{k}', P)
                 # self-attention: [q | k] rows for one GEMM, v as the M operand of the V^T GEMM
                 wq, wk, wv = (_pad_heads_rows(P(f'{t}.attn1.to_{x}.weight'), heads, dh) for x in 'qkv')
-                add_conv(t + '.attn1.qk', torch.cat([wq, wk]))
+                wb.add_gemm(t + '.attn1.qk', torch.cat([wq, wk]))
                 wb.add(t + '.attn1.v:w', G.split_planes(wv))
-                add_conv(t + '.attn1.out', _pad_heads_cols(P(t + '.attn1.to_out.0.weight'), heads, dh), bias=P(t + '.attn1.to_out.0.bias'))
+                wb.add_gemm(t + '.attn1.out', _pad_heads_cols(P(t + '.attn1.to_out.0.weight'), heads, dh), bias=P(t + '.attn1.to_out.0.bias'))
                 # cross-attention
-                add_conv(t + '.attn2.q', _pad_heads_rows(P(t + '.attn2.to_q.weight'), heads, dh), as_f8=f8_linear)
-                add_conv(t + '.attn2.k', _pad_heads_rows(P(t + '.attn2.to_k.weight'), heads, dh))
+                wb.add_gemm(t + '.attn2.q', _pad_heads_rows(P(t + '.attn2.to_q.weight'), heads, dh), f8=f8_linear)
+                wb.add_gemm(t + '.attn2.k', _pad_heads_rows(P(t + '.attn2.to_k.weight'), heads, dh))
                 wb.add(t + '.attn2.v:w', G.split_planes(_pad_heads_rows(P(t + '.attn2.to_v.weight'), heads, dh)))
-                add_conv(t + '.attn2.out', _pad_heads_cols(P(t + '.attn2.to_out.0.weight'), heads, dh), bias=P(t + '.attn2.to_out.0.bias'))
+                wb.add_gemm(t + '.attn2.out', _pad_heads_cols(P(t + '.attn2.to_out.0.weight'), heads, dh), bias=P(t + '.attn2.to_out.0.bias'))
                 info['ctx_dim'] = P(t + '.attn2.to_k.weight').shape[1]
-                add_conv(t + '.ff1', P(t + '.ff.net.0.proj.weight'), bias=P(t + '.ff.net.0.proj.bias'), as_f8=f8_linear)
-                add_conv(t + '.ff2', P(t + '.ff.net.2.weight'), bias=P(t + '.ff.net.2.bias'), as_f8=f8_linear)
-                add_conv(n + '.proj_out', P(n + '.proj_out.weight').reshape(ch, heads * dh), bias=P(n + '.proj_out.bias'), as_f8=f8_linear)
+                wb.add_gemm(t + '.ff1', P(t + '.ff.net.0.proj.weight'), bias=P(t + '.ff.net.0.proj.bias'), f8=f8_linear)
+                wb.add_gemm(t + '.ff2', P(t + '.ff.net.2.weight'), bias=P(t + '.ff.net.2.bias'), f8=f8_linear)
+                wb.add_gemm(n + '.proj_out', P(n + '.proj_out.weight').reshape(ch, heads * dh), bias=P(n + '.proj_out.bias'), f8=f8_linear)
             elif kind == 'qkv_attn':
                 _, _, ch, heads, dh = L
-                wb.add_norm(n + '.norm', P)
                 wqk, bqk, wv, bv = _legacy_qkv_split(P(n + '.qkv.weight').reshape(3 * ch, ch), P(n + '.qkv.bias'), heads, head_pairs)
-                add_conv(n + '.qk', wqk, bias=bqk)
-                wb.add(n + '.v:w', G.split_planes(wv))
-                wb.add(n + '.v:b', bv)
-                add_conv(n + '.proj_out', _legacy_proj_cols(P(n + '.proj_out.weight').reshape(ch, ch), heads, head_pairs),
-                         bias=P(n + '.proj_out.bias'))
+                wproj = _legacy_proj_cols(P(n + '.proj_out.weight').reshape(ch, ch), heads, head_pairs)
+                wb.add_attn_block(n, P, n + '.norm', (wqk, bqk), (wv, bv), (wproj, P(n + '.proj_out.bias')))
             elif kind == 'down':
-                add_conv(n, P(n + '.op.weight'), bias=P(n + '.op.bias'))
+                wb.add_gemm(n, P(n + '.op.weight'), bias=P(n + '.op.bias'))
             elif kind == 'up':
-                add_conv(n, P(n + '.conv.weight'), bias=P(n + '.conv.bias'), as_f8=f8)
+                wb.add_gemm(n, P(n + '.conv.weight'), bias=P(n + '.conv.bias'), f8=f8)
     wb.add('affine:w', torch.cat(aff_w, dim=0))
     wb.add('affine:b', torch.cat(aff_b, dim=0))
     info['aff_total'] = aff_off
     wb.add_norm('out.0', P)
-    add_conv('out.2', P('out.2.weight'), bias=P('out.2.bias'))
+    wb.add_gemm('out.2', P('out.2.weight'), bias=P('out.2.bias'))
     return wb, info
 
 
@@ -214,21 +197,16 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
     CTX = context [Bt, 77, ctx_dim] (nets with cross-attention only), D = eps [Bt,C,R,R] (NCHW), BOTTLENECK = channel-mean of the
     middle block [Bt, 64]."""
     assert nT in (1, Bt)
-    assert not f8 or (npass == 3 and info['f8_shift'])
+    assert not f8 or (npass == 3 and wb.f8_shift)
     assert f8 or not f8_linear
-    fmt_res = 1 if f8 else 0
     fmt_lin = 1 if f8_linear else 0
-
-    def f8_args(key):
-        return dict(f8=True, acc_scale=2.0 ** -info['f8_shift'][key]) if key in info['f8_shift'] else {}
-    pb = PlanBuilder(wb, Bt, npass)
+    pb = PlanBuilder(wb, Bt, npass, f8=f8)
     emit, W = pb.emit, wb.ref
     mc, ted = st['model_channels'], st['ted']
     cd = info['ctx_dim']
     T = ctx_tokens
     TP = CTX_TOKENS_PITCH
-    pb.stats(sum(2 if L[0] == 'res' else (1 if L[0] in ('attn', 'qkv_attn') else 0) for _, ls in st['inp'] + st['mid'] + st['out'] for L in ls)
-             + 1)
+    pb.stats()
     # ---------------- timestep embedding (util.py:151-171, openaimodel.py:723-724) + all emb_layers in one launch -------------
     pb.need('emb0', nT * mc * F4)
     pb.need('e1', nT * ted * F4)
@@ -250,30 +228,7 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
         pb.need('ctx', NPL * Bt * T * cd * H2)
         pb.to_planes(io(S.DS_IO_CTX), cd, T, 1, Bt, 'ctx')
 
-    def lower_res(L, parts, H):
-        """ResBlock (openaimodel.py:255-275): GN+SiLU+conv3x3, + Linear(SiLU(emb)), GN+SiLU+conv3x3, + skip (identity | 1x1)."""
-        _, n, cin, cout = L
-        M = Bt * H * H
-        assert sum(c for _, c in parts) == cin
-        pb.need('act', NPL * M * max(cin, cout) * H2)
-        has_skip = (n + '.c1:w') in wb.off and cin != cout
-        if has_skip:
-            pb.need('raw', NPL * M * cin * H2)
-        pb.group_norm(parts, H, n + '.n0', 1e-5, 'act', raw='raw' if has_skip else None, fmt=fmt_res)
-        pb.need('y', M * cout * F4)
-        off = aff_off[n]
-        emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, cin, W(n + '.c0:w'), cout, taps=9, npass=npass, out_f32=R_('y'), bias=W(n + '.c0:b'),
-                                    rowvec=R_('aff', off * F4), rowvec_stride=aff_stride, **f8_args(n + '.c0'))[0])
-        pb.group_norm([('y', cout)], H, n + '.n1', 1e-5, 'act', fmt=fmt_res)
-        out = pb.need('h:' + n, M * cout * F4)
-        res_name = None if has_skip else parts[0][0]
-        assert has_skip or len(parts) == 1
-        emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, cout, W(n + '.c1:w'), cout, taps=9, npass=npass, a2_ptr=R_('raw') if has_skip else 0,
-                                    C2=cin if has_skip else 0, out_f32=R_(out), bias=W(n + '.c1:b'), residual=R_(res_name) if res_name else 0,
-                                    ldr=cout, scale=1.0, **f8_args(n + '.c1'))[0])
-        return out, cout
-
-    def lower_attn(L, src, H):
+    def lower_transformer(L, src, H):
         """SpatialTransformer with one BasicTransformerBlock (attention.py:250-261, :211-215)."""
         _, n, ch, heads, dh = L
         t = n + '.transformer_blocks.0'
@@ -286,7 +241,7 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
         for nm in ('t0', 't1', 't2', 't3'):
             pb.need(nm, M * inner * F4)
         emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, ch, W(n + '.proj_in:w'), inner, taps=1, npass=npass, out_f32=R_('t0'),
-                                    bias=W(n + '.proj_in:b'), **f8_args(n + '.proj_in'))[0])
+                                    bias=W(n + '.proj_in:b'), **pb.f8_args(n + '.proj_in'))[0])
         pb.need('ln', NPL * M * inner * H2)
         pb.need('qk', NPL * M * 2 * hp * H2)
         pb.need('vt', NPL * Bt * hp * max(Lq, TP) * H2)
@@ -309,7 +264,7 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
         pb.need('q2', NPL * M * hp * H2)
         pb.need('k2', NPL * Bt * T * hp * H2)
         emit(lambda R_: G.conv_gemm(R_('ln'), Bt, H, H, inner, W(t + '.attn2.q:w'), hp, taps=1, npass=npass, out_h16=R_('q2'),
-                                    **f8_args(t + '.attn2.q'))[0])
+                                    **pb.f8_args(t + '.attn2.q'))[0])
         emit(lambda R_: G.rows_gemm(R_('ctx'), Bt * T, cd, 1, W(t + '.attn2.k:w'), G.padded_rows(hp), cd, 1, cd, num_z=1, nh=1, m_valid=Bt * T,
                                     n_valid=hp, npass=npass, out_h16=R_('k2'), ldo=hp, o_plane=Bt * T * hp)[0])
         pb.vt_gemm(t + '.attn2.v:w', 'ctx', cd, hp, T, TP)
@@ -321,37 +276,15 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
         pb.need('ff', M * 8 * inner * F4)
         pb.need('gg', NPL * M * 4 * inner * H2)
         emit(lambda R_: G.conv_gemm(R_('ln'), Bt, H, H, inner, W(t + '.ff1:w'), 8 * inner, taps=1, npass=npass, out_f32=R_('ff'),
-                                    bias=W(t + '.ff1:b'), **f8_args(t + '.ff1'))[0])
+                                    bias=W(t + '.ff1:b'), **pb.f8_args(t + '.ff1'))[0])
         emit(lambda R_: S.GegluDesc(src=R_('ff'), out=R_('gg'), rows=M, I=4 * inner, nplanes=NPL, fmt=fmt_lin))
         emit(lambda R_: G.conv_gemm(R_('gg'), Bt, H, H, 4 * inner, W(t + '.ff2:w'), inner, taps=1, npass=npass, out_f32=R_('t3'),
-                                    bias=W(t + '.ff2:b'), residual=R_('t2'), ldr=inner, **f8_args(t + '.ff2'))[0])
+                                    bias=W(t + '.ff2:b'), residual=R_('t2'), ldr=inner, **pb.f8_args(t + '.ff2'))[0])
         # ---- proj_out + outer residual
         pb.to_planes('t3', inner, H, H, Bt, 'ln', fmt=fmt_lin)
         out = pb.need('h:' + n, M * ch * F4)
         emit(lambda R_: G.conv_gemm(R_('ln'), Bt, H, H, inner, W(n + '.proj_out:w'), ch, taps=1, npass=npass, out_f32=R_(out),
-                                    bias=W(n + '.proj_out:b'), residual=R_(src), ldr=ch, **f8_args(n + '.proj_out'))[0])
-        return out, ch
-
-    def lower_qkv_attn(L, src, H):
-        """Legacy AttentionBlock (openaimodel.py:310-324): x + proj_out(attention(qkv(GroupNorm(x)))), softmax scale 1/sqrt(d)."""
-        _, n, ch, heads, dh = L
-        pairs = info['head_pairs']
-        hs, dp = (heads + heads % 2, 32) if pairs else (heads, dpad(dh))
-        hp = hs * dp
-        Lq = H * H
-        M = Bt * Lq
-        pb.need('act', NPL * M * ch * H2)
-        pb.group_norm([(src, ch)], H, n + '.norm', 1e-5, 'act', silu=0)
-        pb.need('qk', NPL * M * 2 * hp * H2)
-        pb.need('vt', NPL * Bt * hp * Lq * H2)
-        pb.need('o', NPL * M * hp * H2)
-        emit(lambda R_: G.conv_gemm(R_('act'), Bt, H, H, ch, W(n + '.qk:w'), 2 * hp, taps=1, npass=npass, out_h16=R_('qk'),
-                                    bias=W(n + '.qk:b'))[0])
-        pb.vt_gemm(n + '.v:w', 'act', ch, hp, Lq, Lq, bias=n + '.v:b')
-        pb.attention(flash_attn or pairs, 'qk', 'qk', 'o', hs, Lq, Lq, dp, dh ** -0.5, Lq, pairs=pairs)
-        out = pb.need('h:' + n, M * ch * F4)
-        emit(lambda R_: G.conv_gemm(R_('o'), Bt, H, H, hp, W(n + '.proj_out:w'), ch, taps=1, npass=npass, out_f32=R_(out),
-                                    bias=W(n + '.proj_out:b'), residual=R_(src), ldr=ch)[0])
+                                    bias=W(n + '.proj_out:b'), residual=R_(src), ldr=ch, **pb.f8_args(n + '.proj_out'))[0])
         return out, ch
 
     def lower_down(L, src, H):
@@ -365,15 +298,31 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
                                     s2d=True)[0])
         return out, cout, Ho
 
-    def lower_up(L, src, H):
-        _, n, cin, cout = L
-        Ho = H * 2
-        pb.need('act', NPL * Bt * Ho * Ho * cin * H2)
-        pb.to_planes(src, cin, H, H, Bt, 'act', fmt=fmt_res, resample=2)
-        out = pb.need('h:' + n, Bt * Ho * Ho * cout * F4)
-        emit(lambda R_: G.conv_gemm(R_('act'), Bt, Ho, Ho, cin, W(n + ':w'), cout, taps=9, npass=npass, out_f32=R_(out), bias=W(n + ':b'),
-                                    **f8_args(n))[0])
-        return out, cout, Ho
+    def lower(L, parts, H):
+        """One module of a block over `parts` (the input, and for the first ResBlock of an output block the skip) at H x H:
+        (output buffer, channels, output resolution)."""
+        pb.tag += 1
+        kind, n = L[0], L[1]
+        out = 'h:' + n
+        src = parts[0][0]
+        if kind == 'res':
+            _, _, cin, cout = L
+            pb.res_block(n, parts, H, cout, out, eps=1e-5, skip='conv' if cin != cout else 'identity',
+                         emb=('aff', aff_off[n] * F4), emb_stride=aff_stride)
+            pb.need(out, Bt * H * H * cout * F4)
+            return out, cout, H
+        if kind == 'qkv_attn':
+            _, _, ch, heads, dh = L
+            pairs = info['head_pairs']
+            nh, dp = (heads + heads % 2, 32) if pairs else (heads, dpad(dh))
+            pb.attn_block(n, src, ch, H, out, eps=1e-5, heads=nh, d=dp, scale=dh ** -0.5, fused=flash_attn or pairs, pairs=pairs)
+            return out, ch, H
+        if kind == 'down':
+            return lower_down(L, src, H)
+        if kind == 'up':
+            pb.upsample_conv(n, src, L[2], H, L[3], out)
+            return out, L[3], 2 * H
+        return lower_transformer(L, src, H) + (H,)
 
     # ---------------- input conv --------------------------------------------------------------------------------------------
     cimg = st['in_channels']
@@ -388,47 +337,18 @@ def compile_ldm_plan(st, wb, info, B, Bt, nT, R, npass=3, ctx_tokens=77, flash_a
     hs = [(cur, cur_c)]
     for _, layers in st['inp'][1:]:
         for L in layers:
-            pb.tag += 1
-            if L[0] == 'res':
-                cur, cur_c = lower_res(L, [(cur, cur_c)], H)
-            elif L[0] == 'attn':
-                cur, cur_c = lower_attn(L, cur, H)
-            elif L[0] == 'qkv_attn':
-                cur, cur_c = lower_qkv_attn(L, cur, H)
-            elif L[0] == 'down':
-                cur, cur_c, H = lower_down(L, cur, H)
+            cur, cur_c, H = lower(L, [(cur, cur_c)], H)
         hs.append((cur, cur_c))
     for L in st['mid'][0][1]:
-        pb.tag += 1
-        if L[0] == 'res':
-            cur, cur_c = lower_res(L, [(cur, cur_c)], H)
-        elif L[0] == 'qkv_attn':
-            cur, cur_c = lower_qkv_attn(L, cur, H)
-        else:
-            cur, cur_c = lower_attn(L, cur, H)
+        cur, cur_c, H = lower(L, [(cur, cur_c)], H)
     mid_out, mid_c, mid_H = cur, cur_c, H
     emit(lambda R_: S.ChanmeanDesc(src=R_(mid_out), out=io(S.DS_IO_BOTTLENECK), rows=Bt * mid_H * mid_H, C=mid_c))
     for _, layers in st['out']:
-        sk, sc = hs.pop()
-        first_layer = True
-        for L in layers:
-            pb.tag += 1
-            if L[0] == 'res':
-                parts = [(cur, cur_c), (sk, sc)] if first_layer else [(cur, cur_c)]
-                cur, cur_c = lower_res(L, parts, H)
-            elif L[0] == 'attn':
-                cur, cur_c = lower_attn(L, cur, H)
-            elif L[0] == 'qkv_attn':
-                cur, cur_c = lower_qkv_attn(L, cur, H)
-            elif L[0] == 'up':
-                cur, cur_c, H = lower_up(L, cur, H)
-            first_layer = False
+        sk = hs.pop()
+        for i, L in enumerate(layers):
+            cur, cur_c, H = lower(L, [(cur, cur_c)] + ([sk] if i == 0 else []), H)
     # ---------------- out: GN + SiLU + conv3x3 -> eps (NCHW) -----------------------------------------------------------------
-    pb.tag += 1
-    pb.need('act', NPL * Bt * H * H * cur_c * H2)
-    pb.group_norm([(cur, cur_c)], H, 'out.0', 1e-5, 'act')
-    fin_c = cur_c
-    emit(lambda R_: G.conv_gemm(R_('act'), Bt, R, R, fin_c, W('out.2:w'), st['out_channels'], taps=9, npass=npass, bias=W('out.2:b'),
-                                nchw_out=(st['out_channels'], io(S.DS_IO_D)))[0])
     assert H == R
+    pb.tag += 1
+    pb.head_conv(cur, cur_c, H, 'out.0', 1e-5, 'out.2', st['out_channels'], nchw_out=(st['out_channels'], io(S.DS_IO_D)))
     return pb.finish(B=B, Bt=Bt, nT=nT, npass=npass, ctx_tokens=ctx_tokens)

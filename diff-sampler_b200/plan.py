@@ -38,6 +38,7 @@ class WeightBlob:
         self.chunks = []
         self.off = {}
         self.size = 0
+        self.f8_shift = {}          # GEMM key -> S of its weight packed for the f8 mode (acc_scale 2^-S)
 
     def add(self, name, t):
         t = t.detach().contiguous().cpu()
@@ -52,21 +53,43 @@ class WeightBlob:
 
     def add_gemm(self, key, w, skip_w=None, bias=None, f8=False):
         """Conv2d [Cout, Cin, k, k] or linear [N, K] weight (+ a 1x1 skip weight appended along K) as the packed B operand `key`:w of
-        the GEMM kernel -- fp16 hi/lo planes, or the fp16 + 2 x e4m3 layout of the f8 mode -- and its bias `key`:b.
-        Returns (packed weight, f8 shift or None)."""
+        the GEMM kernel -- fp16 hi/lo planes, or the fp16 + 2 x e4m3 layout of the f8 mode -- and its bias `key`:b."""
         if w.dim() == 2:
             w = w.reshape(w.shape[0], w.shape[1], 1, 1)
-        packed, shift = G.pack_conv_weight_f8(w, skip_w) if f8 else (G.pack_conv_weight(w, skip_w), None)
+        if f8:
+            packed, self.f8_shift[key] = G.pack_conv_weight_f8(w, skip_w)
+        else:
+            packed = G.pack_conv_weight(w, skip_w)
         self.add(key + ':w', packed)
         if bias is not None:
             self.add(key + ':b', bias)
-        return packed, shift
 
     def add_norm(self, key, P, src=None):
         """Norm gain and bias `key`:g / `key`:b from the parameters `src`.weight / `src`.bias (src defaults to key; P: name -> tensor)."""
         src = src or key
         self.add(key + ':g', P(src + '.weight'))
         self.add(key + ':b', P(src + '.bias'))
+
+    def add_res_block(self, key, P, norm0, conv0, norm1, conv1, skip=None, f8=False):
+        """The weights PlanBuilder.res_block reads under `key`, from the parameters named by the other arguments (P: name -> tensor):
+        the GroupNorms `norm0` / `norm1` and the 3x3 convolutions `conv0` / `conv1`; a 1x1 `skip` convolution is appended to conv1
+        along K, its bias folded into conv1's.  f8: both convolutions in the f8 GEMM mode."""
+        self.add_norm(key + '.norm0', P, norm0)
+        self.add_gemm(key + '.conv0', P(conv0 + '.weight'), bias=P(conv0 + '.bias'), f8=f8)
+        self.add_norm(key + '.norm1', P, norm1)
+        bias1 = P(conv1 + '.bias')
+        if skip:
+            bias1 = bias1 + P(skip + '.bias')
+        self.add_gemm(key + '.conv1', P(conv1 + '.weight'), P(skip + '.weight') if skip else None, bias=bias1, f8=f8)
+
+    def add_attn_block(self, key, P, norm, qk, v, proj):
+        """The weights PlanBuilder.attn_block reads under `key`: the GroupNorm parameters `norm` (P: name -> tensor), and the (weight,
+        bias) pairs of the [q heads | k heads] rows, the v rows and the output projection, in the head layout the plan runs."""
+        self.add_norm(key + '.norm', P, norm)
+        self.add_gemm(key + '.qk', qk[0], bias=qk[1])
+        self.add(key + '.v:w', G.split_planes(v[0]))            # [2][N][C]: the M operand of the V^T GEMM
+        self.add(key + '.v:b', v[1])
+        self.add_gemm(key + '.proj', proj[0], bias=proj[1])
 
     def ref(self, name, extra=0):
         return S.ref(S.SPACE_WEIGHTS, self.off[name] + extra)
@@ -99,14 +122,23 @@ class PlanBuilder:
     """Collects one plan over the weight blob `wb` for a batch of B samples.
 
     Arena: named buffers, laid out in the order each name is first needed; a name needed again (scratch shared between layers) is
-    sized to the largest request.  Ops: callables build(R) -> descriptor, materialised by finish() once the arena is laid out;
-    R(name, extra=0) is the arena reference.  Each op is stamped with the current `tag` (None: with its own index)."""
+    sized to the largest request.  The block methods below reserve their scratch as they go, so a caller whose arena must keep another
+    order reserves those names first.  Ops: callables build(R) -> descriptor, materialised by finish() once the arena is laid out;
+    R(name, extra=0) is the arena reference.  Each op is stamped with the current `tag` (None: with its own index).
 
-    def __init__(self, wb, B, npass=3, tag=0):
+    Fixed per plan: f8 -- the GEMMs whose weight was packed for the f8 mode run in it; gn_groups(C) -- the group count of a C-channel
+    GroupNorm; gn_coef -- GroupNorms with a gain over at most 2048 channels get the per-(sample, channel) coefficient table;
+    gn_fuse -- the statistics of a GEMM output come from partial sums its producer stores (need_stats)."""
+
+    def __init__(self, wb, B, npass=3, tag=0, f8=False, gn_groups=lambda c: 32, gn_coef=False, gn_fuse=False):
         self.wb, self.B, self.npass, self.tag = wb, B, npass, tag
+        self.f8, self.gn_groups, self.gn_coef, self.gn_fuse = f8, gn_groups, gn_coef, gn_fuse
         self.sizes = {}
         self.ops = []
-        self._slots = self._n_slots = 0
+        self._slots = 0
+        self.prod_of = {}           # buffer name -> (op index of the GEMM that wrote it, Cout, rows)
+        self.quads_of = {}          # producer op index -> arena name of its partial-sum buffer
+        self.unit_of = {}           # producer op index -> channels per partial (4 = quads, 2 = pairs: some consumer has 6/18/30-channel groups)
 
     def need(self, name, nbytes):
         self.sizes[name] = max(self.sizes.get(name, 0), int(nbytes))
@@ -132,29 +164,96 @@ class PlanBuilder:
         meta.update(n_ops=len(self.ops), n_gemm=sum(1 for op in arr if op.type == S.DS_OP_GEMM))
         return Plan(arr, len(self.ops), total, offsets, meta)
 
+    def is_f8(self, key):
+        """GEMM `key` runs in the f8 mode: an f8 plan, and the weight was packed for it (pack_weights may keep narrow blocks fp16x3)."""
+        return self.f8 and key in self.wb.f8_shift
+
+    def f8_args(self, key):
+        return dict(f8=True, acc_scale=2.0 ** -self.wb.f8_shift[key]) if self.is_f8(key) else {}
+
+    def producer(self, name, cout, m_rows, build):
+        """emit() for the GEMM that writes the fp32 tensor `name` [m_rows][cout]: with gn_fuse, a GroupNorm of `name` has it store
+        partial sums (need_stats)."""
+        pid = len(self.ops)
+        self.prod_of[name] = (pid, cout, m_rows)
+
+        def materialise(R):
+            d = build(R)
+            if pid in self.quads_of:
+                d.st_quads = R(self.quads_of[pid])
+                d.st_unit = self.unit_of[pid]
+            return d
+        self.emit(materialise)
+
     # ---- GroupNorm ------------------------------------------------------------------------------------------------------------
-    def stats(self, n_slots):
-        """The 'stats' buffer: fp64 {sum, sumsq} per (sample, group) for up to n_slots GroupNorms, zeroed by a memset op."""
-        nbytes = n_slots * self.B * 32 * 2 * 8
-        self.need('stats', nbytes)
-        self.emit(lambda R: S.MemsetDesc(ptr=R('stats'), bytes=nbytes))
-        self._n_slots = n_slots
+    def stats(self):
+        """The 'stats' buffer: fp64 {sum, sumsq} per (sample, group), one slot per GroupNorm of the plan, zeroed by a memset op here.
+        Its size is the slots taken once the plan is lowered."""
+        self.need('stats', 0)
+        self.emit(lambda R: S.MemsetDesc(ptr=R('stats'), bytes=self.sizes['stats']))
 
     def stats_slot(self):
         """Byte offset of the next GroupNorm's sums in 'stats'."""
-        assert self._slots < self._n_slots
+        assert 'stats' in self.sizes, 'stats() reserves and zeroes the buffer first'
+        nbytes = self.B * 32 * 2 * 8
         self._slots += 1
-        return (self._slots - 1) * self.B * 32 * 2 * 8
+        self.need('stats', self._slots * nbytes)
+        return (self._slots - 1) * nbytes
 
-    def gn_stats(self, slot, parts, hw, groups=32):
-        """Accumulate the fp64 sums of the (virtually concatenated) fp32 NHWC tensors `parts` = [(arena name, channels), ...]."""
+    def need_stats(self, slot, parts, hw, groups, norm=None, eps=0.0, ada=None, ada_stride=0):
+        """GroupNorm statistics over the (virtually concatenated) fp32 tensors `parts` = [(buffer, channels), ...] into `slot`.
+        gn_fuse: when every part was written by a producer() GEMM, that GEMM also stores, per 32-row slab and channel quad, the partial
+        {sum, sumsq} (ds_gemm_desc.st_quads), and a tiny ds_gn_finalize folds slabs and quads into the fp64 sums gn_apply reads.  The
+        partials are independent of the consumer's grouping, so one buffer per tensor serves both the next block and the decoder block
+        that concatenates it as a skip.  No atomics, no pass over the tensor itself.  Otherwise a gn_stats pass over the tensors.
+        gn_coef and norm (the weight key of the gain / bias, with eps and the adaptive scale `ada`): the finalize also writes the
+        per-(sample, channel) coefficient table y = x * a + b into the scratch buffer 'gncoef' (ds_gn_finalize_desc.coef), which lets
+        gn_apply skip its fp64 prologue and run the persistent variant; returns True when the table is produced."""
+        assert len(parts) <= 2
+        B, W = self.B, self.wb.ref
+        c_total = sum(c for _, c in parts)
+        cpg = c_total // groups
         (n0, c0), (n1, c1) = parts[0], (parts[1] if len(parts) > 1 else (None, 0))
-        self.emit(lambda R: S.GnStatsDesc(src0=R(n0), src1=_resolve(R, n1), C0=c0, C1=c1, HW=hw, B=self.B, groups=groups,
-                                          sums=R('stats', slot)))
+        # partial granularity each producer must write for this consumer: 4 channels (quads) when the groups -- and, for a virtual concat
+        # whose first source does not end on a group boundary, both pieces of the straddling group -- are multiples of 4, else 2 (pairs)
+        rem = c0 % cpg if n1 else 0
+        pieces = [cpg] + ([rem, cpg - rem] if rem else [])
+        unit = 4 if all(p % 4 == 0 for p in pieces) else (2 if all(p % 2 == 0 for p in pieces) else 0)
+        fusable = (self.gn_fuse and hw % 32 == 0 and unit and all(c % unit == 0 for _, c in parts)
+                   and all(name in self.prod_of and self.prod_of[name][1] == c for name, c in parts))
+        want_coef = self.gn_coef and norm is not None and c_total <= 2048     # the persistent gn_apply covers up to 256 eight-channel columns
+        if want_coef:
+            self.need('gncoef', B * c_total * 2 * F4)
+
+        def coef_args(R):
+            if not want_coef:
+                return {}
+            return dict(gamma=W(norm + ':g'), beta=W(norm + ':b'), ada=_resolve(R, ada), ada_stride=ada_stride, eps=eps, HW=hw,
+                        coef=R('gncoef'))
+        if not fusable:
+            self.emit(lambda R: S.GnStatsDesc(src0=R(n0), src1=_resolve(R, n1), C0=c0, C1=c1, HW=hw, B=B, groups=groups,
+                                              sums=R('stats', slot)))
+            if want_coef:       # coefficient table from the sums the separate statistics pass accumulated
+                self.emit(lambda R: S.GnFinalizeDesc(quads0=0, quads1=0, C0=c0, C1=c1, slabs_per_sample=0, B=B, groups=groups,
+                                                     sums=R('stats', slot), **coef_args(R)))
+            return want_coef
+        bufs, pids = [], []
+        for name, c in parts:
+            pid, cout, m_rows = self.prod_of[name]
+            self.unit_of[pid] = min(self.unit_of.get(pid, 4), unit)    # a producer serves all its consumers at the finest unit any needs
+            self.quads_of[pid] = self.need('quads:' + name, (m_rows // 32) * (cout // self.unit_of[pid]) * 2 * F4)
+            bufs.append(self.quads_of[pid])
+            pids.append(pid)
+        # unit_of is final only once the whole net is lowered: read it when the descriptors are materialised
+        self.emit(lambda R: S.GnFinalizeDesc(quads0=R(bufs[0]), quads1=R(bufs[1]) if len(bufs) > 1 else 0, C0=c0, C1=c1,
+                                             slabs_per_sample=hw // 32, B=B, groups=groups, sums=R('stats', slot),
+                                             unit0=self.unit_of[pids[0]], unit1=self.unit_of[pids[1]] if len(pids) > 1 else 4,
+                                             **coef_args(R)))
+        return want_coef
 
     def gn_apply(self, parts, H, norm, eps, out, *, W=None, B=None, groups=32, slot=None, coef=False, silu=1, ada=None, ada_stride=0,
                  resample=0, raw=None, raw_f32=None, fmt=0, phase_pitch=0):
-        """GroupNorm of `parts` (as gn_stats; an input may also be an io reference) with the gain / bias `norm`:g / `norm`:b (+ SiLU)
+        """GroupNorm of `parts` (as need_stats; an input may also be an io reference) with the gain / bias `norm`:g / `norm`:b (+ SiLU)
         into the activation operand `out`: fp16 planes, or the f8 operand image (fmt=1).  The statistics are the sums of stats slot
         `slot`, or the coefficient table 'gncoef' (coef=True).  raw / raw_f32 also receive the input un-normalised (fp16 planes /
         fp32); resample 1 / 2 / 3 = 2x2 average pooling / nearest x2 / space-to-depth (phase_pitch: channels per phase, 0 = C).
@@ -169,11 +268,12 @@ class PlanBuilder:
             ada=_resolve(R, ada), ada_stride=ada_stride, resample=resample, nplanes=NPL, out_act=_resolve(R, out),
             out_raw=_resolve(R, raw), out_raw_f32=_resolve(R, raw_f32), fmt=fmt, pad0=phase_pitch))
 
-    def group_norm(self, parts, H, norm, eps, out, **apply_kw):
-        """GroupNorm from sums: a statistics pass into a fresh stats slot, then gn_apply."""
+    def group_norm(self, parts, H, norm, eps, out, *, ada=None, ada_stride=0, **apply_kw):
+        """GroupNorm (+ SiLU) of `parts` at H x H into `out`: the statistics of a fresh stats slot (need_stats), then gn_apply."""
+        groups = self.gn_groups(sum(c for _, c in parts))
         slot = self.stats_slot()
-        self.gn_stats(slot, parts, H * H)
-        self.gn_apply(parts, H, norm, eps, out, slot=slot, **apply_kw)
+        coef = self.need_stats(slot, parts, H * H, groups, norm, eps, ada, ada_stride)
+        self.gn_apply(parts, H, norm, eps, out, groups=groups, slot=slot, coef=coef, ada=ada, ada_stride=ada_stride, **apply_kw)
 
     def to_planes(self, src, C, H, W, B, dst, fmt=0, resample=0, groups=32, phase_pitch=0):
         """fp32 NHWC -> the fp16 hi/lo planes (or, fmt=1, the f8 operand image) of a GEMM operand, without normalisation."""
@@ -216,6 +316,79 @@ class PlanBuilder:
                                         out_h16=R(out), o_zb=L * C, o_zh=d, ldo=C, o_plane=B * L * C, a_k_valid=Lk, b_k_valid=Lk)[0])
 
 
+    # ---- blocks -----------------------------------------------------------------------------------------------------------------
+    def res_block(self, key, parts, H, cout, out, *, eps, skip, skip_scale=1.0, resample=0, emb=None, ada=None, emb_stride=0):
+        """ResBlock `key` (WeightBlob.add_res_block) over the (virtually concatenated) fp32 NHWC tensors `parts` at H x H: GroupNorm + SiLU
+        (resample 1 / 2: 2x2 average pooling / nearest x2) -> conv3x3 (+ the row vector `emb`) -> GroupNorm (ada: adaptive scale / shift
+        rows) + SiLU -> conv3x3 + skip, times skip_scale, into `out`, which the caller reserves.  skip: 'conv' (1x1, appended along K),
+        'identity' (parts[0]) or 'resample' (the resampled input).  emb_stride: row stride of emb / ada (0: one row for the batch).
+        A resampling GroupNorm gets no coefficient table: gn_apply reads the table only without resample."""
+        B, W = self.B, self.wb.ref
+        cin = sum(c for _, c in parts)
+        Ho = {1: H // 2, 2: 2 * H}.get(resample, H)
+        M = B * Ho * Ho
+        conv0, conv1 = key + '.conv0', key + '.conv1'
+        s0 = self.stats_slot()
+        k0 = self.need_stats(s0, parts, H * H, self.gn_groups(cin), key + '.norm0' if resample == 0 else None, eps)
+        self.need('act', NPL * M * max(cin, cout) * H2)
+        if skip == 'conv':
+            self.need('raw', NPL * M * cin * H2)
+        if skip == 'resample':
+            self.need('rawf', M * cin * F4)
+        self.gn_apply(parts, H, key + '.norm0', eps, 'act', groups=self.gn_groups(cin), slot=s0, coef=k0, resample=resample,
+                      raw='raw' if skip == 'conv' else None, raw_f32='rawf' if skip == 'resample' else None, fmt=int(self.is_f8(conv0)))
+        self.need('y', M * cout * F4)
+        self.producer('y', cout, M, lambda R: G.conv_gemm(R('act'), B, Ho, Ho, cin, W(conv0 + ':w'), cout, taps=9, npass=self.npass,
+                                                          out_f32=R('y'), bias=W(conv0 + ':b'), rowvec=_resolve(R, emb),
+                                                          rowvec_stride=emb_stride, **self.f8_args(conv0))[0])
+        self.group_norm([('y', cout)], Ho, key + '.norm1', eps, 'act', ada=ada, ada_stride=emb_stride if ada else 0,
+                        fmt=int(self.is_f8(conv1)))
+        assert skip != 'identity' or len(parts) == 1
+        residual = {'identity': parts[0][0], 'resample': 'rawf'}.get(skip)
+        self.producer(out, cout, M, lambda R: G.conv_gemm(R('act'), B, Ho, Ho, cout, W(conv1 + ':w'), cout, taps=9, npass=self.npass,
+                                                          a2_ptr=R('raw') if skip == 'conv' else 0, C2=cin if skip == 'conv' else 0,
+                                                          out_f32=R(out), bias=W(conv1 + ':b'), residual=_resolve(R, residual), ldr=cout,
+                                                          scale=skip_scale, **self.f8_args(conv1))[0])
+
+    def attn_block(self, key, src, C, H, out, *, eps, heads, d, scale, fused, pairs=False, skip_scale=1.0):
+        """Attention block `key` (WeightBlob.add_attn_block) over the fp32 NHWC tensor `src` [B][H][H][C]: GroupNorm -> the [q | k] 1x1
+        GEMM and the V^T GEMM -> attention over `heads` heads of width d (attention()) -> 1x1 projection + src, times skip_scale,
+        into `out`."""
+        B, W, L = self.B, self.wb.ref, H * H
+        hp = heads * d
+        self.need('act', NPL * B * L * C * H2)
+        self.group_norm([(src, C)], H, key + '.norm', eps, 'act', silu=0)
+        self.need('qk', NPL * B * L * 2 * hp * H2)
+        self.need('vt', NPL * B * hp * L * H2)
+        self.need('o', NPL * B * L * hp * H2)
+        self.emit(lambda R: G.conv_gemm(R('act'), B, H, H, C, W(key + '.qk:w'), 2 * hp, taps=1, npass=self.npass, out_h16=R('qk'),
+                                        bias=W(key + '.qk:b'))[0])
+        self.vt_gemm(key + '.v:w', 'act', C, hp, L, L, bias=key + '.v:b')
+        self.attention(fused, 'qk', 'qk', 'o', heads, L, L, d, scale, L, pairs=pairs)
+        self.need(out, B * L * C * F4)
+        self.producer(out, C, B * L, lambda R: G.conv_gemm(R('o'), B, H, H, hp, W(key + '.proj:w'), C, taps=1, npass=self.npass,
+                                                           out_f32=R(out), bias=W(key + '.proj:b'), residual=R(src), ldr=C,
+                                                           scale=skip_scale)[0])
+
+    def upsample_conv(self, key, src, cin, H, cout, out):
+        """Nearest x2 upsampling of the fp32 NHWC tensor `src` [B][H][H][cin], then the 3x3 convolution `key` into `out`."""
+        B, W, Ho = self.B, self.wb.ref, 2 * H
+        self.need('act', NPL * B * Ho * Ho * cin * H2)
+        self.to_planes(src, cin, H, H, B, 'act', fmt=int(self.is_f8(key)), resample=2)
+        self.need(out, B * Ho * Ho * cout * F4)
+        self.emit(lambda R: G.conv_gemm(R('act'), B, Ho, Ho, cin, W(key + ':w'), cout, taps=9, npass=self.npass, out_f32=R(out),
+                                        bias=W(key + ':b'), **self.f8_args(key))[0])
+
+    def head_conv(self, src, C, H, norm, eps, key, cout, **epilogue):
+        """GroupNorm + SiLU of the fp32 NHWC tensor `src` [B][H][H][C], then the 3x3 convolution `key` to `cout` channels through
+        conv_gemm's output epilogue `epilogue` (edm=... or nchw_out=...; arena names in it are resolved)."""
+        B, W = self.B, self.wb.ref
+        self.need('act', NPL * B * H * H * C * H2)
+        self.group_norm([(src, C)], H, norm, eps, 'act', fmt=int(self.is_f8(key)))
+        self.emit(lambda R: G.conv_gemm(R('act'), B, H, H, C, W(key + ':w'), cout, taps=9, npass=self.npass, bias=W(key + ':b'),
+                                        **{k: tuple(_resolve(R, x) for x in v) for k, v in epilogue.items()},
+                                        **self.f8_args(key))[0])
+
 def _qkv_split(w, b, heads):
     """Reorder the reference's interleaved qkv channels ([head][c][q|k|v], networks_edm.py:174) into
     [q heads | k heads] rows and separate v rows."""
@@ -233,40 +406,23 @@ def pack_weights(spec, params, f8=False, f8_min_channels=0):
     skip) and the head conv in the fp16 + 2 x e4m3 operand layout of the f8 GEMM mode (csrc/ops.h); everything else keeps fp16 hi/lo
     planes (the attention GEMMs share their operand planes, the stem conv reads the 3-channel input).
     f8_min_channels > 0 keeps blocks with fewer input or output channels in fp16x3: the narrow, high-resolution levels average the e4m3
-    rounding over the fewest terms and dominate the f8 error (FFHQ-64: the 128-channel 64x64 levels, tests/study_fp8_corrections.py)."""
+    rounding over the fewest terms and dominate the f8 error (FFHQ-64: the 128-channel 64x64 levels, tests/study_fp8_corrections.py).
+    Returns (blob, info); info holds nothing the lowering reads (the f8 shifts are in blob.f8_shift)."""
     pf = spec.prefix
     P = lambda k: params[pf + k].detach().float().cpu()
     has = lambda k: (pf + k) in params
     wb = WeightBlob()
-    info = {}
-
-    def add_conv(key, w, skip_w=None, bias=None, as_f8=False):
-        packed, shift = wb.add_gemm(key, w, skip_w, bias, f8=as_f8)
-        info[key] = dict(cout=w.shape[0], f8_shift=shift) if as_f8 else dict(cout=w.shape[0], cout_pad=packed.shape[1], ktot=packed.shape[2])
-
-    add_conv(spec.stem, P(spec.stem + '.weight'), bias=P(spec.stem + '.bias'))
+    wb.add_gemm(spec.stem, P(spec.stem + '.weight'), bias=P(spec.stem + '.bias'))
     aff_w, aff_b = [], []
     for b in spec.enc + spec.dec:
         n = b.name
-        wb.add_norm(n + '.norm0', P)
-        blk_f8 = f8 and min(b.cin, b.cout) >= f8_min_channels
-        add_conv(n + '.conv0', P(n + '.conv0.weight'), bias=P(n + '.conv0.bias'), as_f8=blk_f8)
-        wb.add_norm(n + '.norm1', P)
-        bias1 = P(n + '.conv1.bias')
-        skip_w = None
-        if b.skip == 'conv':
-            skip_w = P(n + '.skip.weight')
-            bias1 = bias1 + P(n + '.skip.bias')
-        add_conv(n + '.conv1', P(n + '.conv1.weight'), skip_w, bias=bias1, as_f8=blk_f8)
+        wb.add_res_block(n, P, n + '.norm0', n + '.conv0', n + '.norm1', n + '.conv1', n + '.skip' if b.skip == 'conv' else None,
+                         f8=f8 and min(b.cin, b.cout) >= f8_min_channels)
         aff_w.append(P(n + '.affine.weight'))
         aff_b.append(P(n + '.affine.bias'))
         if b.heads:
-            wb.add_norm(n + '.norm2', P)
             wqk, bqk, wv, bv = _qkv_split(P(n + '.qkv.weight'), P(n + '.qkv.bias'), b.heads)
-            add_conv(n + '.qk', wqk.reshape(wqk.shape[0], wqk.shape[1], 1, 1), bias=bqk)
-            wb.add(n + '.v:w', G.split_planes(wv))            # [2][C][C] used as the M operand
-            wb.add(n + '.v:b', bv)
-            add_conv(n + '.proj', P(n + '.proj.weight'), bias=P(n + '.proj.bias'))
+            wb.add_attn_block(n, P, n + '.norm2', (wqk, bqk), (wv, bv), (P(n + '.proj.weight'), P(n + '.proj.bias')))
     wb.add('affine:w', torch.cat(aff_w, dim=0))
     wb.add('affine:w16', G.split_planes(torch.cat(aff_w, dim=0)))     # [2][aff_total][emb]: N operand of the batched-embedding GEMM
     wb.add('affine:b', torch.cat(aff_b, dim=0))
@@ -279,101 +435,22 @@ def pack_weights(spec, params, f8=False, f8_min_channels=0):
             wb.add('map_label:b', P('map_label.bias'))
     wb.add_norm(spec.head_norm, P)
     # the head conv has 3 output channels: its cost is reading the A operand, which the f8 layout cuts from 3 to 2 tile loads per 64 channels
-    add_conv(spec.head_conv, P(spec.head_conv + '.weight'), bias=P(spec.head_conv + '.bias'),
-             as_f8=f8 and P(spec.head_conv + '.weight').shape[1] >= f8_min_channels)
-    return wb, info
+    wb.add_gemm(spec.head_conv, P(spec.head_conv + '.weight'), bias=P(spec.head_conv + '.bias'),
+                f8=f8 and P(spec.head_conv + '.weight').shape[1] >= f8_min_channels)
+    return wb, {}
 
 
 def compile_plan(spec, wb, winfo, B, nsig, nlab, npass=3, fuse_stats=True, flash_attn=True, f8=False):
     """Lower the forward pass for batch B.  nsig in {1, B}: number of sigma values (embedding rows);
     nlab in {0, 1, B}: rows of class labels supplied.  f8: the block convolutions run in the f8 GEMM mode (weights must have been
-    packed with pack_weights(f8=True))."""
+    packed with pack_weights(f8=True)).  winfo: pack_weights' info.  Every GroupNorm with a gain reads the coefficient table;
+    fuse_stats: GroupNorm statistics from the GEMM epilogues (PlanBuilder.need_stats)."""
     assert nsig in (1, B) and nlab in (0, 1, B)
     assert not f8 or npass == 3
-
-    def is_f8(key):
-        """This GEMM was packed for the f8 mode (pack_weights decides per block: f8_min_channels)."""
-        return f8 and 'f8_shift' in winfo[key]
-
-    def f8_args(key):
-        return dict(f8=True, acc_scale=2.0 ** -winfo[key]['f8_shift']) if is_f8(key) else {}
-    pb = PlanBuilder(wb, B, npass)
+    pb = PlanBuilder(wb, B, npass, f8=f8, gn_groups=_groups, gn_coef=True, gn_fuse=fuse_stats)
     emit, W = pb.emit, wb.ref
     nE = max(nsig, nlab, 1)
     R0 = spec.img_resolution
-
-    # Fused GroupNorm statistics (fuse_stats=True): the GEMM that writes an fp32 tensor also stores, per 32-row slab and channel
-    # quad, the partial {sum, sumsq} (ds_gemm_desc.st_quads); a tiny ds_gn_finalize per GroupNorm folds slabs and quads into the
-    # fp64 sums gn_apply reads.  The partials are independent of the consumer's grouping, so one buffer per tensor serves both the
-    # next block and the decoder block that concatenates it as a skip.  No atomics, no pass over the tensor itself.
-    prod_of = {}            # buffer name -> (op index of the GEMM that wrote it, Cout, rows)
-    quads_of = {}           # producer op index -> arena name of its quad-partial buffer
-    unit_of = {}            # producer op index -> channels per partial (4 = quads, 2 = pairs: some consumer has 6/18/30-channel groups)
-
-    def emit_producer(name, cout, m_rows, build):
-        pid = len(pb.ops)
-        prod_of[name] = (pid, cout, m_rows)
-
-        def materialise(R):
-            d = build(R)
-            if pid in quads_of:
-                d.st_quads = R(quads_of[pid])
-                d.st_unit = unit_of[pid]
-            return d
-        emit(materialise)
-
-    def need_stats(slot, parts, hw, norm=None, eps=0.0, ada=None, ada_stride=0):
-        """GroupNorm statistics over the (virtually concatenated) fp32 tensors `parts` = [(buffer, channels), ...] for `slot`.
-        norm (the weight key of the gain / bias, with eps and the adaptive scale `ada`) additionally asks for the per-(sample, channel)
-        coefficient table y = x * a + b in the scratch buffer 'gncoef' (ds_gn_finalize_desc.coef), which lets gn_apply skip its fp64
-        prologue and run the persistent variant; returns True when the table is produced."""
-        assert len(parts) <= 2
-        c_total = sum(c for _, c in parts)
-        g = _groups(c_total)
-        cpg = c_total // g
-        (n0, c0), (n1, c1) = parts[0], (parts[1] if len(parts) > 1 else (None, 0))
-        # partial granularity each producer must write for this consumer: 4 channels (quads) when the groups -- and, for a virtual concat
-        # whose first source does not end on a group boundary, both pieces of the straddling group -- are multiples of 4, else 2 (pairs)
-        rem = c0 % cpg if n1 else 0
-        pieces = [cpg] + ([rem, cpg - rem] if rem else [])
-        unit = 4 if all(p % 4 == 0 for p in pieces) else (2 if all(p % 2 == 0 for p in pieces) else 0)
-        fusable = (fuse_stats and hw % 32 == 0 and unit and all(c % unit == 0 for _, c in parts)
-                   and all(name in prod_of and prod_of[name][1] == c for name, c in parts))
-        want_coef = norm is not None and c_total <= 2048        # the persistent gn_apply covers up to 256 eight-channel columns
-        if want_coef:
-            pb.need('gncoef', B * c_total * 2 * F4)
-
-        def coef_args(R):
-            if not want_coef:
-                return {}
-            return dict(gamma=W(norm + ':g'), beta=W(norm + ':b'), ada=_resolve(R, ada), ada_stride=ada_stride, eps=eps, HW=hw,
-                        coef=R('gncoef'))
-        if not fusable:
-            pb.gn_stats(slot, parts, hw, groups=g)
-            if want_coef:       # coefficient table from the sums the separate statistics pass accumulated
-                emit(lambda R: S.GnFinalizeDesc(quads0=0, quads1=0, C0=c0, C1=c1, slabs_per_sample=0, B=B, groups=g, sums=R('stats', slot),
-                                                **coef_args(R)))
-            return want_coef
-        bufs, pids = [], []
-        for name, c in parts:
-            pid, cout, m_rows = prod_of[name]
-            unit_of[pid] = min(unit_of.get(pid, 4), unit)           # a producer serves all its consumers at the finest unit any of them needs
-            quads_of[pid] = pb.need('quads:' + name, (m_rows // 32) * (cout // unit_of[pid]) * 2 * F4)
-            bufs.append(quads_of[pid])
-            pids.append(pid)
-        # unit_of is final only once the whole net is lowered: read it when the descriptors are materialised
-        emit(lambda R: S.GnFinalizeDesc(quads0=R(bufs[0]), quads1=R(bufs[1]) if len(bufs) > 1 else 0, C0=c0, C1=c1,
-                                        slabs_per_sample=hw // 32, B=B, groups=g, sums=R('stats', slot), unit0=unit_of[pids[0]],
-                                        unit1=unit_of[pids[1]] if len(pids) > 1 else 4, **coef_args(R)))
-        return want_coef
-
-    def group_norm(parts, H, norm, eps, silu, fmt=0, ada=None):
-        """GroupNorm (+ SiLU) of `parts` at H x H into 'act'."""
-        slot = pb.stats_slot()
-        ada_stride = aff_stride if ada else 0
-        coef = need_stats(slot, parts, H * H, norm, eps, ada, ada_stride)
-        pb.gn_apply(parts, H, norm, eps, 'act', groups=_groups(sum(c for _, c in parts)), slot=slot, coef=coef, silu=silu, ada=ada,
-                    ada_stride=ada_stride, fmt=fmt)
 
     # ---------------- embedding ----------------------------------------------------------------------------------
     pb.need('coef', nsig * 4 * F4)
@@ -382,7 +459,7 @@ def compile_plan(spec, wb, winfo, B, nsig, nlab, npass=3, fuse_stats=True, flash
     pb.need('e2', nE * spec.emb_channels * F4)
     pb.need('e3', nE * spec.emb_channels * F4)
     pb.need('aff', nE * spec.aff_total * F4)
-    pb.stats(2 * len(spec.enc + spec.dec) + sum(1 for b in spec.enc + spec.dec if b.heads) + 1)
+    pb.stats()
     emit(lambda R: S.PosembDesc(sigma=io(S.DS_IO_SIGMA), nsig=nsig, num_channels=spec.noise_channels,
                                 endpoint=1 if spec.kind == 'song' else 0, swap_sincos=1 if spec.kind == 'song' else 0,
                                 sigma_data=spec.sigma_data, coef=R('coef'), emb=R('emb0'),
@@ -432,90 +509,50 @@ def compile_plan(spec, wb, winfo, B, nsig, nlab, npass=3, fuse_stats=True, flash
     emit(lambda R: S.PrepInputDesc(x=io(S.DS_IO_X), coef=R('coef'), coef_stride=4 if nsig > 1 else 0, B=B, C=spec.img_channels,
                                    HW=HW0, nplanes=NPL, out=R('in_planes')))
     pb.need('x:' + spec.stem, B * HW0 * spec.stem_cout * F4)
-    emit_producer('x:' + spec.stem, spec.stem_cout, B * HW0, lambda R: G.conv_gemm(R('in_planes'), B, R0, R0, 64, W(spec.stem + ':w'), spec.stem_cout, taps=9,
-                                                          npass=npass, out_f32=R('x:' + spec.stem), bias=W(spec.stem + ':b'))[0])
+    pb.producer('x:' + spec.stem, spec.stem_cout, B * HW0, lambda R: G.conv_gemm(R('in_planes'), B, R0, R0, 64, W(spec.stem + ':w'),
+                                                                            spec.stem_cout, taps=9, npass=npass,
+                                                                            out_f32=R('x:' + spec.stem), bias=W(spec.stem + ':b'))[0])
 
-    def lower_block(b, x0, c0, x1, c1):
-        """x0/x1: arena names of the (virtually concatenated) fp32 NHWC inputs."""
+    def lower_block(b, parts):
+        """Block b over the (virtually concatenated) fp32 NHWC inputs `parts`: the ResBlock, then the attention block if it has one."""
         pb.tag += 1
         n = b.name
-        Hi, Ho = b.res_in, b.res_out
-        cin, cout = b.cin, b.cout
-        assert c0 + c1 == cin
-        resample = 1 if b.down else (2 if b.up else 0)
-        Mo = B * Ho * Ho
-        parts = [(x0, c0)] + ([(x1, c1)] if x1 else [])
-        s0 = pb.stats_slot()
-        k0 = need_stats(s0, parts, Hi * Hi, n + '.norm0' if resample == 0 else None, b.eps)
-        pb.need('act', NPL * Mo * max(cin, cout) * H2)
-        want_raw = b.skip == 'conv'
-        want_rawf = b.skip == 'resample'
-        if want_raw:
-            pb.need('raw', NPL * Mo * cin * H2)
-        if want_rawf:
-            pb.need('rawf', Mo * cin * F4)
-        pb.gn_apply(parts, Hi, n + '.norm0', b.eps, 'act', groups=_groups(cin), slot=s0, coef=k0, resample=resample,
-                    raw='raw' if want_raw else None, raw_f32='rawf' if want_rawf else None, fmt=1 if is_f8(n + '.conv0') else 0)
-        pb.need('y', Mo * cout * F4)
-        emit_producer('y', cout, Mo, lambda R: G.conv_gemm(R('act'), B, Ho, Ho, cin, W(n + '.conv0:w'), cout, taps=9, npass=npass, out_f32=R('y'),
-                                                 bias=W(n + '.conv0:b'), rowvec=0 if b.adaptive_scale else R('aff', b.aff_off * F4),
-                                                 rowvec_stride=aff_stride, **f8_args(n + '.conv0'))[0])
-        group_norm([('y', cout)], Ho, n + '.norm1', b.eps, 1, fmt=1 if is_f8(n + '.conv1') else 0,
-                   ada=('aff', b.aff_off * F4) if b.adaptive_scale else None)
-        xout = pb.need('x:' + n, Mo * cout * F4)
-        mid = pb.need('xmid', Mo * cout * F4) if b.heads else xout
-        if b.skip == 'identity':
-            assert x1 is None
-            res_name = x0
-        elif b.skip == 'resample':
-            res_name = 'rawf'
-        else:
-            res_name = None
-        emit_producer(mid, cout, Mo, lambda R: G.conv_gemm(R('act'), B, Ho, Ho, cout, W(n + '.conv1:w'), cout, taps=9, npass=npass,
-                                                 a2_ptr=R('raw') if want_raw else 0, C2=cin if want_raw else 0, out_f32=R(mid),
-                                                 bias=W(n + '.conv1:b'), residual=R(res_name) if res_name else 0, ldr=cout,
-                                                 scale=b.skip_scale, **f8_args(n + '.conv1'))[0])
+        Ho = b.res_out
+        assert sum(c for _, c in parts) == b.cin
+        aff = ('aff', b.aff_off * F4)
+        xout = 'x:' + n
+        mid = 'xmid' if b.heads else xout
+        pb.res_block(n, parts, b.res_in, b.cout, mid, eps=b.eps, skip=b.skip, skip_scale=b.skip_scale,
+                     resample=1 if b.down else (2 if b.up else 0), emb=None if b.adaptive_scale else aff,
+                     ada=aff if b.adaptive_scale else None, emb_stride=aff_stride)
+        pb.need(xout, B * Ho * Ho * b.cout * F4)
         if b.heads:
-            nh = b.heads
-            d = cout // nh
-            L = Ho * Ho
-            group_norm([(mid, cout)], Ho, n + '.norm2', b.eps, 0)
-            pb.need('qk', NPL * B * L * 2 * cout * H2)
-            pb.need('vt', NPL * B * cout * L * H2)
-            pb.need('o', NPL * B * L * cout * H2)
-            emit(lambda R: G.conv_gemm(R('act'), B, Ho, Ho, cout, W(n + '.qk:w'), 2 * cout, taps=1, npass=npass, out_h16=R('qk'),
-                                       bias=W(n + '.qk:b'))[0])
-            pb.vt_gemm(n + '.v:w', 'act', cout, cout, L, L, bias=n + '.v:b')
+            pb.need(mid, B * Ho * Ho * b.cout * F4)
+            d = b.cout // b.heads
             # fused: one kernel per attention layer, the L x L score matrix never leaves the SM; L % 8 == 0 for the V^T row pitch
-            pb.attention(flash_attn and d == 64 and L % 8 == 0, 'qk', 'qk', 'o', nh, L, L, d, 1.0 / math.sqrt(d), L)
-            emit_producer(xout, cout, Mo, lambda R: G.conv_gemm(R('o'), B, Ho, Ho, cout, W(n + '.proj:w'), cout, taps=1, npass=npass, out_f32=R(xout),
-                                                      bias=W(n + '.proj:b'), residual=R(mid), ldr=cout, scale=b.skip_scale)[0])
+            pb.attn_block(n, mid, b.cout, Ho, xout, eps=b.eps, heads=b.heads, d=d, scale=1.0 / math.sqrt(d),
+                          fused=flash_attn and d == 64 and Ho * Ho % 8 == 0, skip_scale=b.skip_scale)
         if n == spec.bottleneck_block:
-            emit(lambda R: S.ChanmeanDesc(src=R(xout), out=io(S.DS_IO_BOTTLENECK), rows=B * Ho * Ho, C=cout))
+            emit(lambda R: S.ChanmeanDesc(src=R(xout), out=io(S.DS_IO_BOTTLENECK), rows=B * Ho * Ho, C=b.cout))
         return xout
 
     # ---------------- encoder / decoder --------------------------------------------------------------------------
     skips = [('x:' + spec.stem, spec.stem_cout)]
     cur, cur_c = 'x:' + spec.stem, spec.stem_cout
     for b in spec.enc:
-        cur = lower_block(b, cur, cur_c, None, 0)
+        cur = lower_block(b, [(cur, cur_c)])
         cur_c = b.cout
         skips.append((cur, cur_c))
     for b in spec.dec:
+        parts = [(cur, cur_c)]
         if b.concat:
             sk, sc = skips.pop()
             assert sc == b.concat
-            cur = lower_block(b, cur, cur_c, sk, sc)
-        else:
-            cur = lower_block(b, cur, cur_c, None, 0)
+            parts.append((sk, sc))
+        cur = lower_block(b, parts)
         cur_c = b.cout
     # ---------------- head: GN -> SiLU -> conv3x3 -> EDM combine ----------------------------------------------------
     pb.tag += 1
-    pb.need('act', NPL * B * HW0 * cur_c * H2)
-    fin_c = cur_c
-    group_norm([(cur, fin_c)], R0, spec.head_norm, spec.head_eps, 1, fmt=1 if is_f8(spec.head_conv) else 0)
-    emit(lambda R: G.conv_gemm(R('act'), B, R0, R0, fin_c, W(spec.head_conv + ':w'), spec.img_channels, taps=9, npass=npass,
-                               bias=W(spec.head_conv + ':b'),
-                               edm=(io(S.DS_IO_X), R('coef'), 4 if nsig > 1 else 0, spec.img_channels, io(S.DS_IO_D)),
-                               **f8_args(spec.head_conv))[0])
+    pb.head_conv(cur, cur_c, R0, spec.head_norm, spec.head_eps, spec.head_conv, spec.img_channels,
+                 edm=(io(S.DS_IO_X), 'coef', 4 if nsig > 1 else 0, spec.img_channels, io(S.DS_IO_D)))
     return pb.finish(B=B, nsig=nsig, nlab=nlab, npass=npass, f8=bool(f8))

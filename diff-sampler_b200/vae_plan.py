@@ -75,23 +75,14 @@ def pack_vae_weights(mods, meta, params):
         if m[0] == 'conv':
             wb.add_gemm(n, P(n + '.weight'), bias=P(n + '.bias'))
         elif m[0] == 'res':
-            wb.add_norm(n + '.n1', P, n + '.norm1')
-            wb.add_gemm(n + '.c1', P(n + '.conv1.weight'), bias=P(n + '.conv1.bias'))
-            wb.add_norm(n + '.n2', P, n + '.norm2')
-            b2, skw = P(n + '.conv2.bias'), None
-            if (n + '.nin_shortcut.weight') in params:
-                skw = P(n + '.nin_shortcut.weight')
-                b2 = b2 + P(n + '.nin_shortcut.bias')
             assert (n + '.conv_shortcut.weight') not in params, '3x3 conv_shortcut is not lowered (SD-v1 uses nin_shortcut)'
-            wb.add_gemm(n + '.c2', P(n + '.conv2.weight'), skw, bias=b2)
+            skip = n + '.nin_shortcut' if (n + '.nin_shortcut.weight') in params else None
+            wb.add_res_block(n, P, n + '.norm1', n + '.conv1', n + '.norm2', n + '.conv2', skip)
         elif m[0] == 'attn':
             c = m[2]
-            wb.add_norm(n + '.norm', P)
             wq, wk, wv = (P(f'{n}.{t}.weight').reshape(c, c) for t in 'qkv')
-            wb.add_gemm(n + '.qk', torch.cat([wq, wk]).reshape(2 * c, c, 1, 1), bias=torch.cat([P(n + '.q.bias'), P(n + '.k.bias')]))
-            wb.add(n + '.v:w', G.split_planes(wv))                       # [2][C][C]: the M operand of the V^T GEMM
-            wb.add(n + '.v:b', P(n + '.v.bias'))
-            wb.add_gemm(n + '.proj', P(n + '.proj_out.weight'), bias=P(n + '.proj_out.bias'))
+            wb.add_attn_block(n, P, n + '.norm', (torch.cat([wq, wk]), torch.cat([P(n + '.q.bias'), P(n + '.k.bias')])),
+                              (wv, P(n + '.v.bias')), (P(n + '.proj_out.weight'), P(n + '.proj_out.bias')))
         elif m[0] == 'up':
             wb.add_gemm(n, P(n + '.conv.weight'), bias=P(n + '.conv.bias'))
     wb.add_norm('norm_out', P, 'decoder.norm_out')
@@ -109,55 +100,7 @@ def compile_vae_plan(mods, meta, wb, B, R, npass=3, quantize=False, debug_indice
         raise ValueError('quantize: this first stage has no codebook (not a VQModelInterface)')
     pb = PlanBuilder(wb, B, npass)
     emit, W = pb.emit, wb.ref
-    pb.stats(sum(2 if m[0] == 'res' else (1 if m[0] == 'attn' else 0) for m in mods) + 1)
-
-    def gn(src, c, H, norm, silu, out, raw=None):
-        """GroupNorm(32, eps 1e-6) (+ swish) of the fp32 NHWC tensor `src` -> fp16 planes `out` (+ raw planes for a 1x1 skip)."""
-        pb.group_norm([(src, c)], H, norm, 1e-6, out, silu=silu, raw=raw)
-
-    def lower_res(m, src, H):
-        _, n, cin, cout = m
-        M = B * H * H
-        has_skip = cin != cout
-        pb.need('act', NPL * M * max(cin, cout) * H2)
-        if has_skip:
-            pb.need('raw', NPL * M * cin * H2)
-        gn(src, cin, H, n + '.n1', 1, 'act', raw='raw' if has_skip else None)
-        pb.need('y', M * cout * F4)
-        emit(lambda R_: G.conv_gemm(R_('act'), B, H, H, cin, W(n + '.c1:w'), cout, taps=9, npass=npass, out_f32=R_('y'), bias=W(n + '.c1:b'))[0])
-        gn('y', cout, H, n + '.n2', 1, 'act')
-        out = pb.need('h:' + n, M * cout * F4)
-        emit(lambda R_: G.conv_gemm(R_('act'), B, H, H, cout, W(n + '.c2:w'), cout, taps=9, npass=npass, a2_ptr=R_('raw') if has_skip else 0,
-                                    C2=cin if has_skip else 0, out_f32=R_(out), bias=W(n + '.c2:b'), residual=0 if has_skip else R_(src),
-                                    ldr=cout)[0])
-        return out, cout
-
-    def lower_attn(m, src, H):
-        _, n, c = m
-        L = H * H
-        M = B * L
-        assert L % 64 == 0, 'attention needs a multiple of 64 positions (K extent of the PV product)'
-        pb.need('act', NPL * M * c * H2)
-        gn(src, c, H, n + '.norm', 0, 'act')
-        pb.need('qk', NPL * M * 2 * c * H2)
-        pb.need('vt', NPL * B * c * L * H2)
-        emit(lambda R_: G.conv_gemm(R_('act'), B, H, H, c, W(n + '.qk:w'), 2 * c, taps=1, npass=npass, out_h16=R_('qk'), bias=W(n + '.qk:b'))[0])
-        pb.vt_gemm(n + '.v:w', 'act', c, c, L, L, bias=n + '.v:b')
-        pb.attention(False, 'qk', 'qk', 'o', 1, L, L, c, float(c) ** -0.5, L)
-        pb.need('o', NPL * M * c * H2)
-        out = pb.need('h:' + n, M * c * F4)
-        emit(lambda R_: G.conv_gemm(R_('o'), B, H, H, c, W(n + '.proj:w'), c, taps=1, npass=npass, out_f32=R_(out), bias=W(n + '.proj:b'),
-                                    residual=R_(src), ldr=c)[0])
-        return out, c
-
-    def lower_up(m, src, H):
-        _, n, c = m
-        Ho = 2 * H
-        pb.need('act', NPL * B * Ho * Ho * c * H2)
-        pb.to_planes(src, c, H, H, B, 'act', resample=2)
-        out = pb.need('h:' + n, B * Ho * Ho * c * F4)
-        emit(lambda R_: G.conv_gemm(R_('act'), B, Ho, Ho, c, W(n + ':w'), c, taps=9, npass=npass, out_f32=R_(out), bias=W(n + ':b'))[0])
-        return out, c, Ho
+    pb.stats()
 
     # ---- z / scale_factor (-> nearest codebook row) -> fp16 planes (channels zero-padded to 64) -> post_quant_conv (1x1) -> conv_in ------
     HW = R * R
@@ -174,24 +117,27 @@ def compile_vae_plan(mods, meta, wb, B, R, npass=3, quantize=False, debug_indice
     cur, cur_c, H = None, None, R
     for m in mods:
         pb.tag += 1
+        out = 'h:' + m[1]
         if m[0] == 'conv':
-            cur = pb.need('h:' + m[1], B * HW * m[3] * F4)
+            cur, cur_c = pb.need(out, B * HW * m[3] * F4), m[3]
             emit(lambda R_, m=m, cur=cur: G.conv_gemm(R_('pq_planes'), B, R, R, 64, W(m[1] + ':w'), m[3], taps=9, npass=npass, out_f32=R_(cur),
                                                       bias=W(m[1] + ':b'))[0])
-            cur_c = m[3]
         elif m[0] == 'res':
-            cur, cur_c = lower_res(m, cur, H)
+            _, n, cin, cout = m
+            pb.res_block(n, [(cur, cin)], H, cout, out, eps=1e-6, skip='conv' if cin != cout else 'identity')
+            cur, cur_c = pb.need(out, B * H * H * cout * F4), cout
         elif m[0] == 'attn':
-            cur, cur_c = lower_attn(m, cur, H)
+            assert H * H % 64 == 0, 'attention needs a multiple of 64 positions (K extent of the PV product)'
+            for name in ('qk', 'vt', 'S', 'P'):       # this plan's arena keeps 'o' after the unfused attention's scores
+                pb.need(name, 0)
+            pb.attn_block(m[1], cur, cur_c, H, out, eps=1e-6, heads=1, d=cur_c, scale=float(cur_c) ** -0.5, fused=False)
+            cur = out
         elif m[0] == 'up':
-            cur, cur_c, H = lower_up(m, cur, H)
+            pb.upsample_conv(m[1], cur, cur_c, H, m[2], out)
+            cur, H = out, 2 * H
     # ---- norm_out + swish + conv_out -> images, NCHW fp32 ----------------------------------------------------------------------------
     pb.tag += 1
-    pb.need('act', NPL * B * H * H * cur_c * H2)
-    gn(cur, cur_c, H, 'norm_out', 1, 'act')
-    fin_c, fin_H = cur_c, H
-    emit(lambda R_: G.conv_gemm(R_('act'), B, fin_H, fin_H, fin_c, W('conv_out:w'), meta['out_ch'], taps=9, npass=npass, bias=W('conv_out:b'),
-                                nchw_out=(meta['out_ch'], io(S.DS_IO_D)))[0])
+    pb.head_conv(cur, cur_c, H, 'norm_out', 1e-6, 'conv_out', meta['out_ch'], nchw_out=(meta['out_ch'], io(S.DS_IO_D)))
     assert H == R * meta['upscale']
     if quantize and debug_indices:
         pb.need('vq_idx', B * HW * 4)                             # last: the other buffers keep the offsets of the plain plan

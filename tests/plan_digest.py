@@ -1,7 +1,7 @@
 """SHA-256 digests of compiled plans: the op array bytes, arena size and layout, plan meta and the weight blob.  Used by
-tests/test_cm_host.py to check that the EDM, LDM, VAE and CLIP plans -- the tiny interpreter variants and the benchmarked ones --
-compile byte for byte as they did before the Consistency-Models lowering (tests/golden/plan_digests.json).  Regenerate that file
-only when a change to those plans is intended:
+tests/test_cm_host.py to check that the EDM, CM, LDM, VAE / VQ, CLIP and optimal-denoiser plans -- the tiny interpreter variants,
+the compile options and the full-size and benchmarked nets -- compile byte for byte as pinned in tests/golden/plan_digests.json.
+Regenerate that file only when a change to those plans is intended:
 
     python tests/plan_digest.py > tests/golden/plan_digests.json
 """
@@ -40,6 +40,69 @@ def _edm_variants():
                     yield f'edm/{name}/f8={int(f8)}/B{B}/s{nsig}/l{nlab}/p{npass}', pl, blob
 
 
+def _edm_options():
+    """compile_plan's unfused GroupNorm statistics and unfused attention, and f8 with the narrow blocks kept in fp16x3."""
+    from diff_sampler_b200 import edm_nets, plan as planner
+    from oracle import edm_oracle as O
+    for name in ('tiny_song', 'tiny_adm'):
+        P, St = O.make_net(name, seed=0, dezero=True)
+        spec = edm_nets.spec_from_params(P, St['img_resolution'], St['img_channels'], St['label_dim'])
+        spec.sigma_data = 0.5
+        wb, info = planner.pack_weights(spec, P)
+        nlab = 2 if spec.label_dim else 0
+        for opt in ('fuse_stats', 'flash_attn'):
+            yield f'edm/{name}/{opt}=0', planner.compile_plan(spec, wb, info, 2, 1, nlab, npass=3, **{opt: False}), wb.bytes()
+        if name == 'tiny_song':
+            wb, info = planner.pack_weights(spec, P, f8=True, f8_min_channels=128)
+            yield f'edm/{name}/f8=1/min128', planner.compile_plan(spec, wb, info, 2, 1, 0, npass=3, f8=True), wb.bytes()
+
+
+def _cm_variants():
+    """The Consistency-Models nets: the tiny setting in fp16x3 and f8, and the full-size LSUN-256 net."""
+    from diff_sampler_b200 import cm_net, plan as planner
+    for setting, tag, B, f8s in ((cm_net.TINY_SETTING, 'tiny', 3, (False, True)), (None, 'lsun256', 2, (False,))):
+        spec, params = cm_net.convert(cm_net.init_state_dict(setting), setting)
+        for f8 in f8s:
+            wb, info = planner.pack_weights(spec, params, f8=f8)
+            yield f'cm/{tag}/f8={int(f8)}/B{B}', planner.compile_plan(spec, wb, info, B, 1, 0, npass=3, f8=f8), wb.bytes()
+
+
+def _uncond_ldm_variants():
+    """The unconditional LDM eps-net with 32-wide heads in pairs and padded to 64, and the full-size LDM-VQ-f4 net at batch 32."""
+    import ldm_uncond_ref as U
+    from diff_sampler_b200 import ldm_plan
+    for name, B, pairs_opts in (('tiny_uncond', 2, (True, False)), ('ldm_vq4', 32, (True,))):
+        P, cfg = U.make_params(name)
+        st = ldm_plan.ldm_structure(P, 8, cfg['num_head_channels'])
+        for pairs in pairs_opts:
+            wb, info = ldm_plan.pack_ldm_weights(st, P, head_pairs=pairs)
+            pl = ldm_plan.compile_ldm_plan(st, wb, info, B, B, B, cfg['img_resolution'])
+            yield f'ldm_uncond/{name}/pairs={int(pairs)}/B{B}', pl, wb.bytes()
+
+
+def _vq_variants():
+    """The VQ decoder without and with the codebook snap (and its index read-out), and the full-size VQ-f4 decoder at 64 -> 256."""
+    import vq_ref as VQ
+    from diff_sampler_b200 import vae_plan
+    for name, B, R, kws in (('tiny_vq', 2, 8, ({}, {'quantize': True}, {'quantize': True, 'debug_indices': True})),
+                            ('vq_f4', 1, 64, ({'quantize': True},))):
+        P, _ = VQ.make_params(name)
+        mods, meta = vae_plan.vae_structure(P)
+        wb = vae_plan.pack_vae_weights(mods, meta, P)
+        for kw in kws:
+            key = f'vq/{name}/B{B}/R{R}/' + (','.join(sorted(kw)) or 'plain')
+            yield key, vae_plan.compile_vae_plan(mods, meta, wb, B, R, **kw), wb.bytes()
+
+
+def _optimal_variants():
+    """The small optimal-denoiser plans (their blob is the dataset: only its layout is part of the plan)."""
+    from diff_sampler_b200 import optimal as OPT
+    for N, D, B, nsig, knn in ((300, 192, 4, 1, 0), (65, 105, 3, 3, 0), (130, 48, 2, 1, 5), (70, 105, 3, 3, 0), (70, 105, 3, 3, 4)):
+        g = OPT._Geometry(N, D)
+        wb, _ = OPT.blob_layout(g)
+        yield f'optimal/N{N}/D{D}/B{B}/s{nsig}/knn{knn}', OPT.compile_plan(g, wb, B, nsig, 1.0, knn=knn), wb.bytes()
+
+
 def _small_variants():
     import torch
     from diff_sampler_b200 import clip_plan, ldm_plan, vae_plan
@@ -74,7 +137,8 @@ def _benchmarked():
 
 def all_digests(benchmarked=True):
     out = {}
-    gens = [_edm_variants(), _small_variants()] + ([_benchmarked()] if benchmarked else [])
+    gens = [_edm_variants(), _edm_options(), _cm_variants(), _uncond_ldm_variants(), _vq_variants(), _optimal_variants(),
+            _small_variants()] + ([_benchmarked()] if benchmarked else [])
     for g in gens:
         for key, pl, blob in g:
             out[key] = digest(pl, blob)

@@ -171,7 +171,8 @@ def test_fullsize_plan_passes_the_launcher_checks(built, full, f8):
 
 
 def test_other_plans_compile_as_before():
-    """EDM / LDM / VAE / CLIP plan variants and the five benchmarked plans: op arrays, arena, meta and weight blobs unchanged."""
+    """EDM / CM / LDM / VAE / VQ / CLIP / optimal-denoiser plan variants and the benchmarked plans: op arrays, arena, meta and weight
+    blobs unchanged."""
     import plan_digest
     want = json.load(open(os.path.join(GOLDEN, 'plan_digests.json')))
     got = plan_digest.all_digests()
