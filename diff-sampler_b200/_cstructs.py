@@ -10,6 +10,8 @@ F32 = C.c_float
 DS_OP_GEMM, DS_OP_GN_STATS, DS_OP_GN_APPLY, DS_OP_SOFTMAX, DS_OP_POSEMB, DS_OP_LINEAR = 1, 2, 3, 4, 5, 6
 DS_OP_PREP_INPUT, DS_OP_CHANMEAN, DS_OP_MEMSET, DS_OP_LAYERNORM, DS_OP_GEGLU, DS_OP_GN_FINALIZE, DS_OP_ATTN, DS_OP_EMBED = 7, 8, 9, 10, 11, 12, 13, 14
 DS_OP_OPT_PREP, DS_OP_OPT_SOFTMAX, DS_OP_OPT_REDUCE, DS_OP_OPT_KNN = 15, 16, 17, 18
+DS_OP_IMG_INPUT, DS_OP_IM2COL, DS_OP_POOL = 19, 20, 21
+DS_POOL_MAX, DS_POOL_AVG, DS_POOL_MEAN = 0, 1, 2
 DS_IO_X, DS_IO_D, DS_IO_SIGMA, DS_IO_LABELS, DS_IO_BOTTLENECK, DS_IO_CTX, DS_IO_COUNT = 0, 1, 2, 3, 4, 5, 6
 DS_M_X0, DS_M_EPS, DS_M_DIV, DS_M_NONE = 0, 1, 2, 3
 DS_F8_SH_A16, DS_F8_SH_LO8, DS_F8_SH_HI8 = 6, 13, 2      # csrc/ops.h: power-of-two operand scales of the f8 GEMM mode
@@ -41,6 +43,7 @@ class GemmDesc(C.Structure):
         ('edm_out', I32), ('edm_x', P), ('edm_coef', P), ('edm_coef_stride', I32), ('edm_C', I32), ('edm_D', P),
         ('st_quads', P),
         ('tap_dh', I32 * 9), ('tap_dw', I32 * 9), ('tap_cb', I32 * 9), ('acc_scale', F32), ('st_unit', I32),
+        ('relu', I32),
     ]
 
 
@@ -120,6 +123,22 @@ class OptKnnDesc(C.Structure):
                 ('B', I32), ('N', I32), ('D', I32), ('nslice', I32), ('k', I32), ('ymax', F32)]
 
 
+class ImgInputDesc(C.Structure):
+    _fields_ = [('src', P), ('out', P), ('sn', I64), ('sc', I64), ('sy', I64), ('sx', I64), ('B', I32), ('C', I32), ('H', I32), ('W', I32),
+                ('Ho', I32), ('Wo', I32)]
+
+
+class Im2colDesc(C.Structure):
+    _fields_ = [('src', P), ('out', P), ('B', I32), ('H', I32), ('W', I32), ('C', I32), ('src_pitch', I32), ('src_c0', I32),
+                ('kh', I32), ('kw', I32), ('sh', I32), ('sw', I32), ('ph', I32), ('pw', I32), ('K64', I32), ('nplanes', I32)]
+
+
+class PoolDesc(C.Structure):
+    _fields_ = [('src', P), ('out_f32', P), ('out_h16', P), ('B', I32), ('H', I32), ('W', I32), ('C', I32), ('src_pitch', I32),
+                ('src_c0', I32), ('out_pitch', I32), ('out_c0', I32), ('k', I32), ('stride', I32), ('pad', I32), ('mode', I32),
+                ('nplanes', I32), ('pad0', I32)]
+
+
 class MemsetDesc(C.Structure):
     _fields_ = [('ptr', P), ('bytes', I64)]
 
@@ -129,7 +148,7 @@ class _OpUnion(C.Union):
                 ('posemb', PosembDesc), ('linear', LinearDesc), ('prep_input', PrepInputDesc), ('chanmean', ChanmeanDesc),
                 ('memset', MemsetDesc), ('layernorm', LayernormDesc), ('geglu', GegluDesc), ('gn_finalize', GnFinalizeDesc), ('attn', AttnDesc),
                 ('embed', EmbedDesc), ('opt_prep', OptPrepDesc), ('opt_softmax', OptSoftmaxDesc), ('opt_reduce', OptReduceDesc),
-                ('opt_knn', OptKnnDesc)]
+                ('opt_knn', OptKnnDesc), ('img_input', ImgInputDesc), ('im2col', Im2colDesc), ('pool', PoolDesc)]
 
 
 class PlanOp(C.Structure):
@@ -141,7 +160,7 @@ SIZEOF_CHECKS = {
     DS_OP_POSEMB: PosembDesc, DS_OP_LINEAR: LinearDesc, DS_OP_PREP_INPUT: PrepInputDesc, DS_OP_CHANMEAN: ChanmeanDesc,
     DS_OP_MEMSET: MemsetDesc, DS_OP_LAYERNORM: LayernormDesc, DS_OP_GEGLU: GegluDesc, DS_OP_GN_FINALIZE: GnFinalizeDesc, DS_OP_ATTN: AttnDesc,
     DS_OP_EMBED: EmbedDesc, DS_OP_OPT_PREP: OptPrepDesc, DS_OP_OPT_SOFTMAX: OptSoftmaxDesc, DS_OP_OPT_REDUCE: OptReduceDesc,
-    DS_OP_OPT_KNN: OptKnnDesc,
+    DS_OP_OPT_KNN: OptKnnDesc, DS_OP_IMG_INPUT: ImgInputDesc, DS_OP_IM2COL: Im2colDesc, DS_OP_POOL: PoolDesc,
 }
 
 # Union member of each op type of the network plans (plan.py, ldm_plan.py, vae_plan.py, clip_plan.py) ...
@@ -152,9 +171,11 @@ UNION_FIELD = {
 }
 # ... and of the ops only the optimal-denoiser plans (optimal.py) use around their two GEMMs.
 OPT_UNION_FIELD = {DS_OP_OPT_PREP: 'opt_prep', DS_OP_OPT_SOFTMAX: 'opt_softmax', DS_OP_OPT_REDUCE: 'opt_reduce', DS_OP_OPT_KNN: 'opt_knn'}
-ALL_UNION_FIELD = {**UNION_FIELD, **OPT_UNION_FIELD}
+# ... and of the ops only the Inception-v3 feature extractor (inception_plan.py) uses around its GEMMs.
+INCEPTION_UNION_FIELD = {DS_OP_IMG_INPUT: 'img_input', DS_OP_IM2COL: 'im2col', DS_OP_POOL: 'pool'}
+ALL_UNION_FIELD = {**UNION_FIELD, **OPT_UNION_FIELD, **INCEPTION_UNION_FIELD}
 OP_TYPE_OF = {GemmDesc: DS_OP_GEMM, GnStatsDesc: DS_OP_GN_STATS, GnApplyDesc: DS_OP_GN_APPLY, SoftmaxDesc: DS_OP_SOFTMAX,
               PosembDesc: DS_OP_POSEMB, LinearDesc: DS_OP_LINEAR, PrepInputDesc: DS_OP_PREP_INPUT, ChanmeanDesc: DS_OP_CHANMEAN,
               MemsetDesc: DS_OP_MEMSET, LayernormDesc: DS_OP_LAYERNORM, GegluDesc: DS_OP_GEGLU, GnFinalizeDesc: DS_OP_GN_FINALIZE, AttnDesc: DS_OP_ATTN,
               EmbedDesc: DS_OP_EMBED, OptPrepDesc: DS_OP_OPT_PREP, OptSoftmaxDesc: DS_OP_OPT_SOFTMAX, OptReduceDesc: DS_OP_OPT_REDUCE,
-              OptKnnDesc: DS_OP_OPT_KNN}
+              OptKnnDesc: DS_OP_OPT_KNN, ImgInputDesc: DS_OP_IMG_INPUT, Im2colDesc: DS_OP_IM2COL, PoolDesc: DS_OP_POOL}

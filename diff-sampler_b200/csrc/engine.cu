@@ -103,6 +103,9 @@ static void visit_ptrs(ds_plan_op& op, F f) {
         case DS_OP_OPT_SOFTMAX: { auto& d = op.u.opt_softmax; P(d.part); P(d.hy2); P(d.xn2); P(d.sigma); P(d.x); P(d.y); P(d.P); P(d.status); break; }
         case DS_OP_OPT_REDUCE: { auto& d = op.u.opt_reduce; P(d.part); P(d.out); break; }
         case DS_OP_OPT_KNN: { auto& d = op.u.opt_knn; P(d.part); P(d.hy2); P(d.xn2); P(d.x); P(d.y); P(d.dist); P(d.idx); break; }
+        case DS_OP_IMG_INPUT: { auto& d = op.u.img_input; P(d.src); P(d.out); break; }
+        case DS_OP_IM2COL: { auto& d = op.u.im2col; P(d.src); P(d.out); break; }
+        case DS_OP_POOL: { auto& d = op.u.pool; P(d.src); P(d.out_f32); P(d.out_h16); break; }
         default: break;
     }
 #undef P
@@ -125,6 +128,9 @@ static dsb::OpCheck check_op(const ds_plan_op& op) {
         case DS_OP_OPT_SOFTMAX: return dsb::opt_softmax_check(op.u.opt_softmax);
         case DS_OP_OPT_REDUCE: return dsb::opt_reduce_check(op.u.opt_reduce);
         case DS_OP_OPT_KNN: return dsb::opt_knn_check(op.u.opt_knn);
+        case DS_OP_IMG_INPUT: return dsb::img_input_check(op.u.img_input);
+        case DS_OP_IM2COL: return dsb::im2col_check(op.u.im2col);
+        case DS_OP_POOL: return dsb::pool_check(op.u.pool);
         case DS_OP_SOFTMAX: case DS_OP_POSEMB: case DS_OP_CHANMEAN: case DS_OP_MEMSET: return {0, nullptr};
         default: return {-100, "unknown op type"};
     }
@@ -150,6 +156,9 @@ static int launch_op(const ds_plan_op& op, const unsigned char* gemm_kp, cudaStr
         case DS_OP_OPT_SOFTMAX: return ds_opt_softmax_launch(&op.u.opt_softmax, s);
         case DS_OP_OPT_REDUCE: return ds_opt_reduce_launch(&op.u.opt_reduce, s);
         case DS_OP_OPT_KNN: return ds_opt_knn_launch(&op.u.opt_knn, s);
+        case DS_OP_IMG_INPUT: return ds_img_input_launch(&op.u.img_input, s);
+        case DS_OP_IM2COL: return ds_im2col_launch(&op.u.im2col, s);
+        case DS_OP_POOL: return ds_pool_launch(&op.u.pool, s);
         case DS_OP_ATTN:
             if (gemm_kp) return dsb::attn_run(reinterpret_cast<const dsb::AttnKernelParams*>(gemm_kp), s);
             return ds_attn_launch(&op.u.attn, s);
@@ -503,6 +512,9 @@ size_t ds_sizeof(int which) {
         case DS_OP_OPT_SOFTMAX: return sizeof(ds_opt_softmax_desc);
         case DS_OP_OPT_REDUCE: return sizeof(ds_opt_reduce_desc);
         case DS_OP_OPT_KNN: return sizeof(ds_opt_knn_desc);
+        case DS_OP_IMG_INPUT: return sizeof(ds_img_input_desc);
+        case DS_OP_IM2COL: return sizeof(ds_im2col_desc);
+        case DS_OP_POOL: return sizeof(ds_pool_desc);
         default: return 0;
     }
 }

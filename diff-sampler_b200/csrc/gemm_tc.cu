@@ -67,6 +67,7 @@ struct alignas(64) GemmKernelParams {
     int tap_dh[9], tap_dw[9], tap_cb[9];
     int f8_last_steps;                   // e4m3 MMAs (K = 32) of the last 128-channel block of a tap: 2 when only its first 64 channels exist
                                          // (C = 64, 192, 576: the other two would multiply TMA zero fill with zero-padded weights), else 4
+    int relu;
 };
 
 struct SmemCtl {
@@ -159,6 +160,10 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKernelParams& p, const 
     }
 #pragma unroll
     for (int j = 0; j < W; ++j) r[j] *= p.scale;
+    if (p.relu) {
+#pragma unroll
+        for (int j = 0; j < W; ++j) r[j] = r[j] > 0.f ? r[j] : 0.f;
+    }
 
     if (p.st_quads) {
         const int lane = threadIdx.x & 31;
@@ -659,6 +664,7 @@ int gemm_build(const ds_gemm_desc* d, GemmKernelParams* kp) {
     kp->st_quads = d->st_quads;
     kp->st_unit = d->st_unit == 2 ? 2 : 4;
     kp->acc_scale = d->acc_scale == 0.f ? 1.f : d->acc_scale;
+    kp->relu = d->relu != 0;
     if (d->f8 & 1) {
         // e4m3 correction passes: byte planes behind the fp16 plane of each operand (layout: csrc/ops.h)
         const int64_t C = d->a_dims[0], Wd = d->a_dims[1], Hd = d->a_dims[2], Bn = d->a_plane_n;

@@ -96,6 +96,7 @@ typedef struct ds_gemm_desc {
     int32_t st_unit;        // channels per statistics partial of st_quads: 4 (default; 0 is read as 4) or 2 (channel PAIRS, for consumers whose
                             // GroupNorm groups are even but not multiples of 4 channels: the 6-, 18-, 30-channel groups of the ADM net);
                             // layout st_quads[((row/32) * (n_valid/unit) + channel/unit) * 2 + {0,1}]
+    int32_t relu;           // 1: v = max(v, 0) after bias / residual / scale, before the statistics and every store (Inception's BasicConv2d)
 } ds_gemm_desc;
 
 int ds_gemm_launch(const ds_gemm_desc* d, cudaStream_t stream);
@@ -415,6 +416,57 @@ typedef struct ds_opt_knn_desc {
     float ymax;
 } ds_opt_knn_desc;
 
+// ---------------------------------------------------------------------------------------------
+// Inception-v3 FID feature extractor (inception.cu; the TF graph `inception-2015-12-05` as DESIGN.md 4.10 states it).  Every
+// convolution runs on the GEMM kernel (rows mode, relu = 1); these ops feed it and pool between its launches.
+//
+// Input stage: uint8 images (element (n, c, y, x) at n*sn + c*sc + y*sy + x*sx, so NCHW and the NHWC-permuted view both fit) ->
+// TF1 legacy ResizeBilinear to Ho x Wo (source (i H / Ho, j W / Wo), neighbours floor and floor + 1 clamped to H-1 / W-1, no half-pixel
+// centres, no antialiasing) -> (v - 128) / 128 as fp32 NHWC [B][Ho][Wo][C].  Coordinates and weights in fp64.
+typedef struct ds_img_input_desc {
+    const unsigned char* src;
+    float* out;
+    int64_t sn, sc, sy, sx;     // element strides of src
+    int32_t B, C, H, W;
+    int32_t Ho, Wo;
+} ds_img_input_desc;
+
+// im2col: fp32 NHWC [B][H][W][src_pitch], channels src_c0 .. src_c0 + C -> fp16 planes [nplanes][B*Ho*Wo][K64] (hi, then lo at
+// + B*Ho*Wo*K64 elements), row (n, oy, ox), column (i*kw + j)*C + c = src(n, oy*sh - ph + i, ox*sw - pw + j, c), 0 outside the image,
+// and columns kh*kw*C .. K64 - 1 zero.  Ho = (H + 2 ph - kh) / sh + 1, Wo likewise.
+typedef struct ds_im2col_desc {
+    const float* src;
+    void* out;
+    int32_t B, H, W, C;
+    int32_t src_pitch, src_c0;
+    int32_t kh, kw, sh, sw, ph, pw;
+    int32_t K64;
+    int32_t nplanes;        // 1 or 2
+} ds_im2col_desc;
+
+// Pooling over fp32 NHWC [B][H][W][src_pitch], channels src_c0 .. src_c0 + C, k x k window, stride, pad:
+//   mode 0 max (padding never wins), 1 average over the window's in-image pixels only (count_include_pad=False),
+//   2 global mean over H x W (k, stride, pad unused): out_f32 [B][out_pitch] at channel out_c0.
+// Modes 0 / 1 write fp32 [B][Ho][Wo][out_pitch] and / or fp16 planes [nplanes][B*Ho*Wo][out_pitch] (lo at + B*Ho*Wo*out_pitch), both
+// at channel out_c0; Ho = (H + 2 pad - k) / stride + 1.
+enum { DS_POOL_MAX = 0, DS_POOL_AVG = 1, DS_POOL_MEAN = 2 };
+typedef struct ds_pool_desc {
+    const float* src;
+    float* out_f32;         // may be NULL (modes 0 / 1)
+    void* out_h16;          // may be NULL; modes 0 / 1 only
+    int32_t B, H, W, C;
+    int32_t src_pitch, src_c0;
+    int32_t out_pitch, out_c0;
+    int32_t k, stride, pad;
+    int32_t mode;
+    int32_t nplanes;        // 1 or 2 (out_h16)
+    int32_t pad0;
+} ds_pool_desc;
+
+int ds_img_input_launch(const ds_img_input_desc* d, cudaStream_t stream);
+int ds_im2col_launch(const ds_im2col_desc* d, cudaStream_t stream);
+int ds_pool_launch(const ds_pool_desc* d, cudaStream_t stream);
+
 int ds_opt_prep_launch(const ds_opt_prep_desc* d, cudaStream_t stream);
 int ds_opt_softmax_launch(const ds_opt_softmax_desc* d, cudaStream_t stream);
 int ds_opt_reduce_launch(const ds_opt_reduce_desc* d, cudaStream_t stream);
@@ -445,7 +497,7 @@ int ds_embed_launch(const ds_embed_desc* d, cudaStream_t stream);
 enum { DS_OP_GEMM = 1, DS_OP_GN_STATS = 2, DS_OP_GN_APPLY = 3, DS_OP_SOFTMAX = 4, DS_OP_POSEMB = 5, DS_OP_LINEAR = 6,
        DS_OP_PREP_INPUT = 7, DS_OP_CHANMEAN = 8, DS_OP_MEMSET = 9, DS_OP_LAYERNORM = 10, DS_OP_GEGLU = 11,
        DS_OP_GN_FINALIZE = 12, DS_OP_ATTN = 13, DS_OP_EMBED = 14, DS_OP_OPT_PREP = 15, DS_OP_OPT_SOFTMAX = 16,
-       DS_OP_OPT_REDUCE = 17, DS_OP_OPT_KNN = 18 };
+       DS_OP_OPT_REDUCE = 17, DS_OP_OPT_KNN = 18, DS_OP_IMG_INPUT = 19, DS_OP_IM2COL = 20, DS_OP_POOL = 21 };
 enum { DS_IO_X = 0, DS_IO_D = 1, DS_IO_SIGMA = 2, DS_IO_LABELS = 3, DS_IO_BOTTLENECK = 4, DS_IO_CTX = 5, DS_IO_COUNT = 6 };
 
 typedef struct ds_memset_desc {
@@ -475,6 +527,9 @@ typedef struct ds_plan_op {
         ds_opt_softmax_desc opt_softmax;
         ds_opt_reduce_desc opt_reduce;
         ds_opt_knn_desc opt_knn;
+        ds_img_input_desc img_input;
+        ds_im2col_desc im2col;
+        ds_pool_desc pool;
     } u;
 } ds_plan_op;
 
@@ -503,5 +558,8 @@ OpCheck opt_prep_check(const ds_opt_prep_desc& d);
 OpCheck opt_softmax_check(const ds_opt_softmax_desc& d);
 OpCheck opt_reduce_check(const ds_opt_reduce_desc& d);
 OpCheck opt_knn_check(const ds_opt_knn_desc& d);
+OpCheck img_input_check(const ds_img_input_desc& d);
+OpCheck im2col_check(const ds_im2col_desc& d);
+OpCheck pool_check(const ds_pool_desc& d);
 }  // namespace dsb
 #endif

@@ -159,10 +159,10 @@ def conv_gemm(a_ptr, Bn, H, W, C, w_ptr, Cout, *, taps=9, npass=3, a_planes=2, w
 def rows_gemm(a_ptr, a_rows, a_pitch, a_batches, b_ptr, b_rows, b_pitch, b_batches, K, *, num_z, nh=1, m_valid, n_valid,
               npass=3, a_planes=2, b_planes=2, a_c_per_zh=0, a_n_per_zb=0, a_n_per_zh=0, b_k0=0, b_k_per_zh=0, b_row_per_zh=0,
               b_z_per_zb=0, b_z_per_zh=0, out_f32=0, out_h16=0, o_zb=0, o_zh=0, ldo=0, o_plane=0, bias_n=0, bias_m=0,
-              residual=0, ldr=0, scale=1.0, bn=None, a_k_valid=None, b_k_valid=None):
+              residual=0, ldr=0, scale=1.0, bn=None, a_k_valid=None, b_k_valid=None, relu=0):
     """Batched row-major product  D_z[m][n] = sum_k A_z[m][k] * B_z[n][k].
     A: fp16 planes [a_planes][a_batches][a_rows][a_pitch]; B: fp16 planes [b_planes][b_batches][b_rows][b_pitch].
-    z = zb*nh + zh selects the batch entry / column window of each operand (see csrc/ops.h)."""
+    z = zb*nh + zh selects the batch entry / column window of each operand (see csrc/ops.h).  relu=1: max(v, 0) before the stores."""
     assert K % 64 == 0
     d = S.GemmDesc()
     BN, n_tiles = (bn, -(-n_valid // bn)) if bn else fill_bn(n_valid, -(-m_valid // 128), num_z)
@@ -194,6 +194,7 @@ def rows_gemm(a_ptr, a_rows, a_pitch, a_batches, b_ptr, b_rows, b_pitch, b_batch
     d.rows_per_sample = 1
     d.residual, d.ldr = residual, ldr
     d.scale = scale
+    d.relu = relu
     return d, dict(BN=BN, n_tiles=n_tiles)
 
 
