@@ -11,6 +11,8 @@ DS_OP_GEMM, DS_OP_GN_STATS, DS_OP_GN_APPLY, DS_OP_SOFTMAX, DS_OP_POSEMB, DS_OP_L
 DS_OP_PREP_INPUT, DS_OP_CHANMEAN, DS_OP_MEMSET, DS_OP_LAYERNORM, DS_OP_GEGLU, DS_OP_GN_FINALIZE, DS_OP_ATTN, DS_OP_EMBED = 7, 8, 9, 10, 11, 12, 13, 14
 DS_OP_OPT_PREP, DS_OP_OPT_SOFTMAX, DS_OP_OPT_REDUCE, DS_OP_OPT_KNN = 15, 16, 17, 18
 DS_OP_IMG_INPUT, DS_OP_IM2COL, DS_OP_POOL = 19, 20, 21
+DS_OP_CLIP_INPUT, DS_OP_CLIP_HEAD = 22, 23
+DS_CLIP_GATHER, DS_CLIP_L2NORM, DS_CLIP_SCORE = 0, 1, 2
 DS_POOL_MAX, DS_POOL_AVG, DS_POOL_MEAN = 0, 1, 2
 DS_IO_X, DS_IO_D, DS_IO_SIGMA, DS_IO_LABELS, DS_IO_BOTTLENECK, DS_IO_CTX, DS_IO_COUNT = 0, 1, 2, 3, 4, 5, 6
 DS_M_X0, DS_M_EPS, DS_M_DIV, DS_M_NONE = 0, 1, 2, 3
@@ -139,6 +141,16 @@ class PoolDesc(C.Structure):
                 ('nplanes', I32), ('pad0', I32)]
 
 
+class ClipInputDesc(C.Structure):
+    _fields_ = [('src', P), ('tab', P), ('out', P), ('sn', I64), ('sc', I64), ('sy', I64), ('sx', I64), ('B', I32), ('H', I32), ('W', I32),
+                ('S', I32), ('ky', I32), ('kx', I32), ('mean', F32 * 3), ('std', F32 * 3)]
+
+
+class ClipHeadDesc(C.Structure):
+    _fields_ = [('src', P), ('src2', P), ('ids', P), ('out', P), ('src_stride', I64), ('out_stride', I64), ('B', I32), ('C', I32), ('T', I32),
+                ('row', I32), ('mode', I32), ('scale', F32)]
+
+
 class MemsetDesc(C.Structure):
     _fields_ = [('ptr', P), ('bytes', I64)]
 
@@ -148,7 +160,8 @@ class _OpUnion(C.Union):
                 ('posemb', PosembDesc), ('linear', LinearDesc), ('prep_input', PrepInputDesc), ('chanmean', ChanmeanDesc),
                 ('memset', MemsetDesc), ('layernorm', LayernormDesc), ('geglu', GegluDesc), ('gn_finalize', GnFinalizeDesc), ('attn', AttnDesc),
                 ('embed', EmbedDesc), ('opt_prep', OptPrepDesc), ('opt_softmax', OptSoftmaxDesc), ('opt_reduce', OptReduceDesc),
-                ('opt_knn', OptKnnDesc), ('img_input', ImgInputDesc), ('im2col', Im2colDesc), ('pool', PoolDesc)]
+                ('opt_knn', OptKnnDesc), ('img_input', ImgInputDesc), ('im2col', Im2colDesc), ('pool', PoolDesc),
+                ('clip_input', ClipInputDesc), ('clip_head', ClipHeadDesc)]
 
 
 class PlanOp(C.Structure):
@@ -161,6 +174,7 @@ SIZEOF_CHECKS = {
     DS_OP_MEMSET: MemsetDesc, DS_OP_LAYERNORM: LayernormDesc, DS_OP_GEGLU: GegluDesc, DS_OP_GN_FINALIZE: GnFinalizeDesc, DS_OP_ATTN: AttnDesc,
     DS_OP_EMBED: EmbedDesc, DS_OP_OPT_PREP: OptPrepDesc, DS_OP_OPT_SOFTMAX: OptSoftmaxDesc, DS_OP_OPT_REDUCE: OptReduceDesc,
     DS_OP_OPT_KNN: OptKnnDesc, DS_OP_IMG_INPUT: ImgInputDesc, DS_OP_IM2COL: Im2colDesc, DS_OP_POOL: PoolDesc,
+    DS_OP_CLIP_INPUT: ClipInputDesc, DS_OP_CLIP_HEAD: ClipHeadDesc,
 }
 
 # Union member of each op type of the network plans (plan.py, ldm_plan.py, vae_plan.py, clip_plan.py) ...
@@ -173,9 +187,12 @@ UNION_FIELD = {
 OPT_UNION_FIELD = {DS_OP_OPT_PREP: 'opt_prep', DS_OP_OPT_SOFTMAX: 'opt_softmax', DS_OP_OPT_REDUCE: 'opt_reduce', DS_OP_OPT_KNN: 'opt_knn'}
 # ... and of the ops only the Inception-v3 feature extractor (inception_plan.py) uses around its GEMMs.
 INCEPTION_UNION_FIELD = {DS_OP_IMG_INPUT: 'img_input', DS_OP_IM2COL: 'im2col', DS_OP_POOL: 'pool'}
-ALL_UNION_FIELD = {**UNION_FIELD, **OPT_UNION_FIELD, **INCEPTION_UNION_FIELD}
+# ... and of the ops only the CLIP-score towers (openclip_plan.py) add.
+OPENCLIP_UNION_FIELD = {DS_OP_CLIP_INPUT: 'clip_input', DS_OP_CLIP_HEAD: 'clip_head'}
+ALL_UNION_FIELD = {**UNION_FIELD, **OPT_UNION_FIELD, **INCEPTION_UNION_FIELD, **OPENCLIP_UNION_FIELD}
 OP_TYPE_OF = {GemmDesc: DS_OP_GEMM, GnStatsDesc: DS_OP_GN_STATS, GnApplyDesc: DS_OP_GN_APPLY, SoftmaxDesc: DS_OP_SOFTMAX,
               PosembDesc: DS_OP_POSEMB, LinearDesc: DS_OP_LINEAR, PrepInputDesc: DS_OP_PREP_INPUT, ChanmeanDesc: DS_OP_CHANMEAN,
               MemsetDesc: DS_OP_MEMSET, LayernormDesc: DS_OP_LAYERNORM, GegluDesc: DS_OP_GEGLU, GnFinalizeDesc: DS_OP_GN_FINALIZE, AttnDesc: DS_OP_ATTN,
               EmbedDesc: DS_OP_EMBED, OptPrepDesc: DS_OP_OPT_PREP, OptSoftmaxDesc: DS_OP_OPT_SOFTMAX, OptReduceDesc: DS_OP_OPT_REDUCE,
-              OptKnnDesc: DS_OP_OPT_KNN, ImgInputDesc: DS_OP_IMG_INPUT, Im2colDesc: DS_OP_IM2COL, PoolDesc: DS_OP_POOL}
+              OptKnnDesc: DS_OP_OPT_KNN, ImgInputDesc: DS_OP_IMG_INPUT, Im2colDesc: DS_OP_IM2COL, PoolDesc: DS_OP_POOL,
+              ClipInputDesc: DS_OP_CLIP_INPUT, ClipHeadDesc: DS_OP_CLIP_HEAD}

@@ -55,8 +55,75 @@ def pack_clip_weights(params, cfg):
     return wb
 
 
-def compile_clip_plan(cfg, wb, B, T, num_heads=None, eps=1e-5, npass=3):
-    """Lower the text encoder for B prompts of T tokens (T <= max_position_embeddings)."""
+ACTS = {'quick_gelu': 1, 'gelu': 2}      # ds_geglu_desc.mode of the MLP activation: CLIPTextModel's quick-GELU, open_clip's exact GELU
+
+
+def reserve_layer_buffers(pb, M, H, I, keys_pitch):
+    """The arena scratch of transformer_layer for M = B x T token rows of width H and MLP width I (call before the first layer; the
+    text plan's arena order is h0, h1, ln, qk, vt, o, ff, gg)."""
+    B = pb.B
+    pb.need('h0', M * H * F4)
+    pb.need('h1', M * H * F4)
+    pb.need('ln', NPL * M * H * H2)
+    pb.need('qk', NPL * M * 2 * H * H2)
+    pb.need('vt', NPL * B * H * keys_pitch * H2)
+    pb.need('o', NPL * M * H * H2)
+    pb.need('ff', M * I * F4)
+    pb.need('gg', NPL * M * I * H2)
+
+
+def layernorm(pb, src, key, out, rows, C, eps, fmt=0):
+    """LayerNorm of the fp32 rows `src` with the gain / bias `key`:g / `key`:b into `out` (an arena name or a reference): fp16 planes, or
+    fp32 with fmt=2."""
+    W = pb.wb.ref
+    pb.emit(lambda R: S.LayernormDesc(src=R(src), gamma=W(key + ':g'), beta=W(key + ':b'), out=R(out) if isinstance(out, str) else out,
+                                      rows=rows, C=C, nplanes=NPL, eps=eps, fmt=fmt))
+
+
+def linear(pb, a, M, K, key, N, bias=True, **kw):
+    """[M][K] activation planes `a` x packed weight `key`:w [N][K] (+ bias `key`:b) through the batched-rows GEMM form; keyword values
+    that are callables are resolved against the arena."""
+    W = pb.wb.ref
+    pb.emit(lambda R: G.rows_gemm(R(a), M, K, 1, W(key + ':w'), G.padded_rows(N), K, 1, K, num_z=1, nh=1, m_valid=M, n_valid=N,
+                                  npass=pb.npass, bias_n=W(key + ':b') if bias else 0, ldo=N,
+                                  **{k: (v(R) if callable(v) else v) for k, v in kw.items()})[0])
+
+
+def transformer_layer(pb, key, M, T, H, I, nh, hd, keys_pitch, eps, causal, act):
+    """One pre-LN residual attention block over the stream 'h0' [M = B x T][H] fp32 (CLIPEncoderLayer; open_clip
+    ResidualAttentionBlock), back into 'h0':
+        h1 = h0 + out(attention(LN1(h0)))        [q | k] one GEMM, V^T one GEMM, fused attention with nh heads of width hd
+        h0 = h1 + fc2(act(fc1(LN2(h1))))         act: 'quick_gelu' or 'gelu' (exact erf)
+    Weights under `key`: .qk (q rows then k rows), .v:w / .v:b, .out, .fc1, .fc2, .layer_norm1, .layer_norm2."""
+    layernorm(pb, 'h0', key + '.layer_norm1', 'ln', M, H, eps)
+    linear(pb, 'ln', M, H, key + '.qk', 2 * H, out_h16=lambda R: R('qk'), o_plane=M * 2 * H)
+    pb.vt_gemm(key + '.v:w', 'ln', H, H, T, keys_pitch, bias=key + '.v:b')
+    pb.attention(True, 'qk', 'qk', 'o', nh, T, T, hd, hd ** -0.5, keys_pitch, causal=causal)
+    linear(pb, 'o', M, H, key + '.out', H, out_f32=lambda R: R('h1'), residual=lambda R: R('h0'), ldr=H)
+    layernorm(pb, 'h1', key + '.layer_norm2', 'ln', M, H, eps)
+    linear(pb, 'ln', M, H, key + '.fc1', I, out_f32=lambda R: R('ff'))
+    pb.emit(lambda R: S.GegluDesc(src=R('ff'), out=R('gg'), rows=M, I=I, nplanes=NPL, fmt=0, mode=ACTS[act]))
+    linear(pb, 'gg', M, I, key + '.fc2', H, out_f32=lambda R: R('h0'), residual=lambda R: R('h1'), ldr=H)
+
+
+def pooled_head(pb, src, src_stride, C, norm, proj, E, eps, ids=None, row=0):
+    """One row per sample of the fp32 stream `src` (sample n at n * src_stride floats: the row argmax(ids[n]) of the token ids `ids`, or
+    `row`) -> LayerNorm `norm` -> @ the projection `proj`:w [E][C] (no bias) -> L2-normalised into io D [B][E] fp32."""
+    B = pb.B
+    pb.need('pool', B * C * F4)
+    pb.need('pool16', NPL * B * C * H2)
+    pb.need('emb', B * E * F4)
+    pb.emit(lambda R: S.ClipHeadDesc(src=R(src), ids=ids or 0, out=R('pool'), src_stride=src_stride, out_stride=C, B=B, C=C,
+                                     T=src_stride // C, row=row, mode=S.DS_CLIP_GATHER))
+    layernorm(pb, 'pool', norm, 'pool16', B, C, eps)
+    linear(pb, 'pool16', B, C, proj, E, bias=False, out_f32=lambda R: R('emb'))
+    pb.emit(lambda R: S.ClipHeadDesc(src=R('emb'), out=io(S.DS_IO_D), B=B, C=E, mode=S.DS_CLIP_L2NORM))
+
+
+def compile_clip_plan(cfg, wb, B, T, num_heads=None, eps=1e-5, npass=3, act='quick_gelu', prefix='', proj_dim=None):
+    """Lower the text encoder for B prompts of T tokens (T <= max_position_embeddings).  Weights under `prefix` (tok, pos, l<i>.*,
+    final).  proj_dim=None: last_hidden_state into io D; else the pooled text embedding of open_clip's encode_text, L2-normalised: the
+    final LayerNorm of the row at argmax(ids) @ `prefix`proj [proj_dim][H] into io D [B][proj_dim]."""
     H, I = cfg['hidden_size'], cfg['intermediate_size']
     nh = num_heads or cfg.get('num_attention_heads') or H // 64
     if H != nh * 64:
@@ -65,38 +132,14 @@ def compile_clip_plan(cfg, wb, B, T, num_heads=None, eps=1e-5, npass=3):
         raise ValueError(f'{T} tokens exceed the position table ({cfg["max_position_embeddings"]})')
     M = B * T
     pb = PlanBuilder(wb, B, npass, tag=None)           # each op tagged with its index
-    emit, W = pb.emit, wb.ref
-    pb.need('h0', M * H * F4)
-    pb.need('h1', M * H * F4)
-    pb.need('ln', NPL * M * H * H2)
-    pb.need('qk', NPL * M * 2 * H * H2)
-    pb.need('vt', NPL * B * H * KEYS_PITCH * H2)
-    pb.need('o', NPL * M * H * H2)
-    pb.need('ff', M * I * F4)
-    pb.need('gg', NPL * M * I * H2)
-
-    def layernorm(src, g, b, out, fmt=0):
-        emit(lambda R_: S.LayernormDesc(src=R_(src), gamma=W(g), beta=W(b), out=out(R_), rows=M, C=H, nplanes=NPL, eps=eps, fmt=fmt))
-
-    def linear(a, K, key, N, **kw):
-        """[M][K] activation planes x packed weight [N][K] (+ bias[N]) through the batched-rows GEMM form."""
-        emit(lambda R_: G.rows_gemm(R_(a), M, K, 1, W(key + ':w'), G.padded_rows(N), K, 1, K, num_z=1, nh=1, m_valid=M, n_valid=N, npass=npass,
-                                    bias_n=W(key + ':b'), ldo=N, **{k: (v(R_) if callable(v) else v) for k, v in kw.items()})[0])
-
-    emit(lambda R_: S.EmbedDesc(ids=io(S.DS_IO_X), tok=W('tok'), pos=W('pos'), out=R_('h0'), rows=M, T=T, C=H, vocab=cfg['vocab_size']))
+    W = wb.ref
+    reserve_layer_buffers(pb, M, H, I, KEYS_PITCH)
+    pb.emit(lambda R_: S.EmbedDesc(ids=io(S.DS_IO_X), tok=W(prefix + 'tok'), pos=W(prefix + 'pos'), out=R_('h0'), rows=M, T=T, C=H,
+                                   vocab=cfg['vocab_size']))
     for i in range(cfg['num_hidden_layers']):
-        L = f'l{i}'
-        # ---- h1 = h0 + out_proj(causal_attention(LN1(h0)))
-        layernorm('h0', L + '.layer_norm1:g', L + '.layer_norm1:b', lambda R_: R_('ln'))
-        linear('ln', H, L + '.qk', 2 * H, out_h16=lambda R_: R_('qk'), o_plane=M * 2 * H)
-        pb.vt_gemm(L + '.v:w', 'ln', H, H, T, KEYS_PITCH, bias=L + '.v:b')
-        pb.attention(True, 'qk', 'qk', 'o', nh, T, T, 64, 64 ** -0.5, KEYS_PITCH, causal=1)
-        linear('o', H, L + '.out', H, out_f32=lambda R_: R_('h1'), residual=lambda R_: R_('h0'), ldr=H)
-        # ---- h0 = h1 + fc2(quick_gelu(fc1(LN2(h1))))
-        layernorm('h1', L + '.layer_norm2:g', L + '.layer_norm2:b', lambda R_: R_('ln'))
-        linear('ln', H, L + '.fc1', I, out_f32=lambda R_: R_('ff'))
-        emit(lambda R_: S.GegluDesc(src=R_('ff'), out=R_('gg'), rows=M, I=I, nplanes=NPL, fmt=0, mode=1))
-        linear('gg', I, L + '.fc2', H, out_f32=lambda R_: R_('h0'), residual=lambda R_: R_('h1'), ldr=H)
-    layernorm('h0', 'final:g', 'final:b', lambda R_: io(S.DS_IO_D), fmt=2)
-
+        transformer_layer(pb, f'{prefix}l{i}', M, T, H, I, nh, 64, KEYS_PITCH, eps, causal=1, act=act)
+    if proj_dim is None:
+        layernorm(pb, 'h0', prefix + 'final', io(S.DS_IO_D), M, H, eps, fmt=2)
+    else:
+        pooled_head(pb, 'h0', T * H, H, prefix + 'final', prefix + 'proj', proj_dim, eps, ids=io(S.DS_IO_X))
     return pb.finish(B=B, T=T, npass=npass)

@@ -1,4 +1,5 @@
-// Fused softmax attention for sm_90a (head dim padded to 64; 32-wide heads in pairs: attn_pair_kernel): O = softmax(scale * Q K^T) V
+// Fused softmax attention for sm_90a (head dim padded to 64; 32-wide heads in pairs: attn_pair_kernel; 72..128-wide heads:
+// attn_wide_kernel): O = softmax(scale * Q K^T) V
 // without materialising the L x Lk score matrix in HBM.  Reference: diff-solvers-main/models/networks_edm.py:105-118 (AttentionOp) / :174-178 (UNetBlock attention),
 // models/ldm/modules/attention.py:152-196 (CrossAttention.forward).
 //
@@ -44,6 +45,7 @@ struct alignas(64) AttnKernelParams {
     int o_pitch;
     int causal;                 // query l sees keys <= l
     int pair;                   // attn_pair_kernel: 32-wide heads, nh counts head pairs
+    int hd;                     // attn_wide_kernel: the head width (72 .. 128); 0 for the other kernels
 };
 
 struct AttnCtl {
@@ -391,15 +393,190 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_pair_kernel(const __grid
     }
 }
 
+// Heads of width hd = 72 .. 128, a multiple of 8 (ds_attn_desc.pad0 = hd; open_clip ViT-g-14: 16 heads of 88).  One head per CTA as
+// attn_kernel, with every head-width extent read as 128 channels through 4-D tensor maps that carry the head as its own dimension:
+//   Q, K   {hd, nh, L | Lk, 2B}, boxes {64, 1, rows, 1} at channels 0 and 64 of the head: two 64-channel swizzle atoms per row
+//   V^T    {keys, hd, nh, 2B}, box {64 keys, 128 d-rows, 1, 1}
+// TMA zero-fills channels (V^T rows) hd .. 127, so no GEMM pads its output to 128 and the zero channels add nothing to S or O.  S takes
+// ceil(hd / 16) k16 steps per pass; O is two m64n64k16 accumulators (d-rows 0..63, 64..127), of which the store keeps columns < hd.
+// Q is 64 KB and a K + V^T stage 64 KB, so the ring has 2 stages.  O[64] accumulates in the wgmma itself (alpha-scaled first, no
+// per-block accumulator as in attn_kernel): that keeps S, P and O within the 168 registers of a 384-thread CTA without a stack frame;
+// with at most a few hundred keys the tensor cores' accumulation error stays at the level of one key block.
+static constexpr int kWideStages = 2;
+static constexpr int kWideQBytes = 4 * 16384;      // Q hi, lo: 2 channel blocks x 128 rows x 64 fp16 each
+static constexpr int kWideKBytes = 4 * 8192;       // K hi, lo: 2 channel blocks x 64 keys x 64
+static constexpr int kWideVBytes = 2 * 16384;      // V^T hi, lo: 128 d-rows x 64 keys
+static constexpr int kWideStageBytes = kWideKBytes + kWideVBytes;
+static constexpr int kWideOffCtl = kWideQBytes + kWideStages * kWideStageBytes;
+static constexpr size_t kWideSmem = kWideOffCtl + 256 + 1024;
+static_assert(kWideSmem <= 227 * 1024, "attn_wide_kernel shared memory");
+
+__global__ void __launch_bounds__(kAttnThreads, 1) attn_wide_kernel(const __grid_constant__ AttnKernelParams p) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    AttnCtl* ctl = reinterpret_cast<AttnCtl*>(smem + kWideOffCtl);
+
+    const int wg = threadIdx.x >> 7;
+    const int qt = blockIdx.x % p.q_tiles;
+    const int z = blockIdx.x / p.q_tiles;
+    const int h = z % p.nh;
+    const int b = z / p.nh;
+    const int nkv = (p.Lk + 63) >> 6;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&p.tmQ);
+        tma_prefetch_desc(&p.tmK);
+        tma_prefetch_desc(&p.tmV);
+        mbar_init(&ctl->q_full, 1);
+        for (int s = 0; s < kWideStages; ++s) {
+            mbar_init(&ctl->kv_full[s], 1);
+            mbar_init(&ctl->kv_empty[s], 2);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
+            mbar_arrive_expect_tx(&ctl->q_full, kWideQBytes);
+            for (int pl = 0; pl < 2; ++pl)
+                for (int cb = 0; cb < 2; ++cb)
+                    tma_load_4d(&p.tmQ, &ctl->q_full, smem + pl * 32768 + cb * 16384, cb * 64, h, qt * 128, pl * p.B + b);
+            for (int j = 0; j < nkv; ++j) {
+                const int s = j % kWideStages;
+                mbar_wait(&ctl->kv_empty[s], ((j / kWideStages) & 1) ^ 1);
+                mbar_arrive_expect_tx(&ctl->kv_full[s], kWideStageBytes);
+                uint8_t* sk = smem + kWideQBytes + s * kWideStageBytes;
+                for (int pl = 0; pl < 2; ++pl) {
+                    for (int cb = 0; cb < 2; ++cb)
+                        tma_load_4d(&p.tmK, &ctl->kv_full[s], sk + pl * 16384 + cb * 8192, cb * 64, h, j * 64, pl * p.B + b);
+                    tma_load_4d(&p.tmV, &ctl->kv_full[s], sk + kWideKBytes + pl * 16384, j * 64, 0, h, pl * p.B + b);
+                }
+            }
+        }
+        return;
+    }
+
+    const int cw = wg - 1;
+    const int lane = threadIdx.x & 31;
+    const int w = (threadIdx.x >> 5) & 3;
+    const int r0 = cw * 64 + 16 * w + (lane >> 2);
+    const int q0 = qt * 128 + r0;
+    const uint32_t sq = smem_u32(smem) + cw * 64 * 128;
+    float O[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) O[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+
+    mbar_wait(&ctl->q_full, 0);
+    for (int j = 0; j < nkv; ++j) {
+        const int s = j % kWideStages;
+        mbar_wait(&ctl->kv_full[s], (j / kWideStages) & 1);
+        const uint32_t sk = smem_u32(smem + kWideQBytes + s * kWideStageBytes);
+        const uint32_t sv = sk + kWideKBytes;
+        // Q descriptors are rebuilt per block rather than hoisted out of the key loop: kept live, they would be spilled
+        uint32_t sqj = sq;
+        asm volatile("" : "+r"(sqj));
+        float S[32];
+        wgmma_fence();
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+#pragma unroll
+            for (int cb = 0; cb < 2; ++cb) {
+                const uint64_t da = wgmma_desc_sw128(sqj + (pass == 1 ? 32768 : 0) + cb * 16384);
+                const uint64_t db = wgmma_desc_sw128(sk + (pass == 2 ? 16384 : 0) + cb * 8192);
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    Wgmma<64>::f16(S, da + 2 * k, db + 2 * k, (pass > 0 || cb > 0 || k > 0) ? 1u : 0u);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(S);
+
+        const int kv = p.Lk - j * 64;                   // keys of this block: column c valid iff c < kv
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+            const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+            if (col < kv) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], S[i]);
+        }
+        float alpha[2], mn[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+            mn[hr] = fmaxf(m[hr], mx[hr] * p.scale_log2e);
+            alpha[hr] = m[hr] == -INFINITY ? 0.f : ex2_approx(m[hr] - mn[hr]);     // O and l are still zero before the first block
+        }
+        uint32_t Ph[16], Pl[16];
+        float ls[2] = {0.f, 0.f};
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+            const int hr = (i >> 1) & 1;
+            const int col = 8 * (i >> 2) + 2 * (lane & 3);
+            const float p0 = col < kv ? ex2_approx(fmaf(S[i], p.scale_log2e, -mn[hr])) : 0.f;
+            const float p1 = col + 1 < kv ? ex2_approx(fmaf(S[i + 1], p.scale_log2e, -mn[hr])) : 0.f;
+            ls[hr] += p0 + p1;
+            split_h16_pair(p0, p1, Ph[i >> 1], Pl[i >> 1]);
+        }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            l[hr] = l[hr] * alpha[hr] + ls[hr];
+            m[hr] = mn[hr];
+        }
+#pragma unroll
+        for (int i = 0; i < 64; ++i) O[i] *= alpha[(i >> 1) & 1];
+        // O += P V: the two correction passes (Pl V_hi, Ph V_lo) first; d-rows 64 c .. 64 c + 63 of V^T are 8 KB into the tile
+        wgmma_fence();
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+            const uint32_t* A = pass == 0 ? Pl : Ph;
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const uint64_t db = wgmma_desc_sw128(sv + (pass == 1 ? 16384 : 0) + c * 8192);
+#pragma unroll
+                for (int kc = 0; kc < 4; ++kc) wgmma_f16_rs_n64(O + 32 * c, A + 4 * kc, db + 2 * kc);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(O);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&ctl->kv_empty[s]);
+    }
+
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 1);
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        const int grow = q0 + 8 * hr;
+        if (grow >= p.L) continue;
+        const float inv = 1.f / l[hr];
+        __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * p.hd + 2 * (lane & 3);
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+                const float v[2] = {O[32 * c + 4 * g + 2 * hr] * inv, O[32 * c + 4 * g + 2 * hr + 1] * inv};
+                if (64 * c + 8 * g < p.hd) store_planes<2>(o, p.o_plane, 64 * c + 8 * g, v, 2);   // hd % 8 == 0: whole 8-column groups
+            }
+    }
+}
+
 // ------------------------------------------------------------------------------------------ host
 // Width of each head: pad0 of the descriptor (0 = 64).
 static int attn_head_dim(const ds_attn_desc& d) { return d.pad0 == 0 ? 64 : d.pad0; }
+static bool attn_wide(int hd) { return hd >= 72 && hd <= 128 && hd % 8 == 0; }
 
 OpCheck attn_check(const ds_attn_desc& d) {
     if (d.nplanes != 2 || d.B <= 0 || d.nh <= 0 || d.L <= 0 || d.Lk <= 0 || !(d.scale > 0.f)) return {-30, "attn: args"};
     if (d.q_pitch % 8 || d.k_pitch % 8 || d.vt_pitch % 8 || d.o_pitch % 8 || d.q_c0 % 8 || d.k_c0 % 8) return {-31, "attn: pitch"};
     const int hd = attn_head_dim(d);
-    if (hd != 64 && hd != 32) return {-41, "attn: head_dim"};
+    if (hd != 64 && hd != 32 && !attn_wide(hd)) return {-41, "attn: head_dim"};
+    if (attn_wide(hd) && d.causal) return {-43, "attn: wide causal"};     // the wide kernel has no causal mask (CLIP text heads are 64 wide)
     // 32-wide heads run in pairs (one 64-channel box): an odd head count is padded with a zero head by the plan
     if (hd == 32 && d.nh % 2) return {-42, "attn: pair head count"};
     if (d.q_c0 + d.nh * hd > d.q_pitch || d.k_c0 + d.nh * hd > d.k_pitch || d.nh * hd > d.o_pitch || d.Lk > d.vt_pitch)
@@ -410,24 +587,41 @@ OpCheck attn_check(const ds_attn_desc& d) {
 
 int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
     if (const int rc = attn_check(*d).rc) return rc;
-    {
-        const int64_t dims[3] = {d->q_pitch, d->L, (int64_t)2 * d->B};
-        const int64_t str[2] = {(int64_t)d->q_pitch * 2, (int64_t)d->L * d->q_pitch * 2};
-        const int32_t box[3] = {64, 128, 1};
-        if (encode_map(&kp->tmQ, d->q, 3, dims, str, box)) return -33;
-    }
-    {
-        const int64_t dims[3] = {d->k_pitch, d->Lk, (int64_t)2 * d->B};
-        const int64_t str[2] = {(int64_t)d->k_pitch * 2, (int64_t)d->Lk * d->k_pitch * 2};
-        const int32_t box[3] = {64, 64, 1};
-        if (encode_map(&kp->tmK, d->k, 3, dims, str, box)) return -34;
-    }
-    {
-        const int64_t rows = (int64_t)d->nh * attn_head_dim(*d);
-        const int64_t dims[3] = {d->Lk, rows, (int64_t)2 * d->B};
-        const int64_t str[2] = {(int64_t)d->vt_pitch * 2, rows * d->vt_pitch * 2};
-        const int32_t box[3] = {64, 64, 1};
-        if (encode_map(&kp->tmV, d->vt, 3, dims, str, box)) return -35;
+    const int hd = attn_head_dim(*d);
+    kp->hd = attn_wide(hd) ? hd : 0;
+    if (kp->hd) {
+        const int64_t qdims[4] = {hd, d->nh, d->L, (int64_t)2 * d->B};
+        const int64_t qstr[3] = {(int64_t)hd * 2, (int64_t)d->q_pitch * 2, (int64_t)d->L * d->q_pitch * 2};
+        const int32_t qbox[4] = {64, 1, 128, 1};
+        if (encode_map(&kp->tmQ, static_cast<const __half*>(d->q) + d->q_c0, 4, qdims, qstr, qbox)) return -33;
+        const int64_t kdims[4] = {hd, d->nh, d->Lk, (int64_t)2 * d->B};
+        const int64_t kstr[3] = {(int64_t)hd * 2, (int64_t)d->k_pitch * 2, (int64_t)d->Lk * d->k_pitch * 2};
+        const int32_t kbox[4] = {64, 1, 64, 1};
+        if (encode_map(&kp->tmK, static_cast<const __half*>(d->k) + d->k_c0, 4, kdims, kstr, kbox)) return -34;
+        const int64_t vdims[4] = {d->Lk, hd, d->nh, (int64_t)2 * d->B};
+        const int64_t vstr[3] = {(int64_t)d->vt_pitch * 2, (int64_t)hd * d->vt_pitch * 2, (int64_t)d->nh * hd * d->vt_pitch * 2};
+        const int32_t vbox[4] = {64, 128, 1, 1};
+        if (encode_map(&kp->tmV, d->vt, 4, vdims, vstr, vbox)) return -35;
+    } else {
+        {
+            const int64_t dims[3] = {d->q_pitch, d->L, (int64_t)2 * d->B};
+            const int64_t str[2] = {(int64_t)d->q_pitch * 2, (int64_t)d->L * d->q_pitch * 2};
+            const int32_t box[3] = {64, 128, 1};
+            if (encode_map(&kp->tmQ, d->q, 3, dims, str, box)) return -33;
+        }
+        {
+            const int64_t dims[3] = {d->k_pitch, d->Lk, (int64_t)2 * d->B};
+            const int64_t str[2] = {(int64_t)d->k_pitch * 2, (int64_t)d->Lk * d->k_pitch * 2};
+            const int32_t box[3] = {64, 64, 1};
+            if (encode_map(&kp->tmK, d->k, 3, dims, str, box)) return -34;
+        }
+        {
+            const int64_t rows = (int64_t)d->nh * attn_head_dim(*d);
+            const int64_t dims[3] = {d->Lk, rows, (int64_t)2 * d->B};
+            const int64_t str[2] = {(int64_t)d->vt_pitch * 2, rows * d->vt_pitch * 2};
+            const int32_t box[3] = {64, 64, 1};
+            if (encode_map(&kp->tmV, d->vt, 3, dims, str, box)) return -35;
+        }
     }
     kp->pair = attn_head_dim(*d) == 32 ? 1 : 0;
     kp->B = d->B; kp->nh = kp->pair ? d->nh / 2 : d->nh; kp->L = d->L; kp->Lk = d->Lk; kp->q_c0 = d->q_c0; kp->k_c0 = d->k_c0;
@@ -443,19 +637,21 @@ int attn_build(const ds_attn_desc* d, AttnKernelParams* kp) {
 size_t attn_params_size() { return sizeof(AttnKernelParams); }
 
 int attn_run(const AttnKernelParams* kp, cudaStream_t stream) {
-    static bool attr_set[64][2] = {};               // per device (cudaFuncSetAttribute is a per-device setting) and kernel
+    static bool attr_set[64][3] = {};               // per device (cudaFuncSetAttribute is a per-device setting) and kernel
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) return -39;
-    const int pr = kp->pair ? 1 : 0;
-    if (!attr_set[dev][pr]) {
-        if (cudaFuncSetAttribute(pr ? attn_pair_kernel : attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmem) != cudaSuccess)
-            return -36;
-        attr_set[dev][pr] = true;
+    const int kind = kp->hd ? 2 : (kp->pair ? 1 : 0);
+    const size_t smem = kind == 2 ? kWideSmem : kAttnSmem;
+    if (!attr_set[dev][kind]) {
+        const void* fn = kind == 2 ? (const void*)attn_wide_kernel : (kind == 1 ? (const void*)attn_pair_kernel : (const void*)attn_kernel);
+        if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -36;
+        attr_set[dev][kind] = true;
     }
     const long long grid = (long long)kp->B * kp->nh * kp->q_tiles;
     if (grid <= 0 || grid > 0x7fffffffLL) return -37;
-    if (pr) attn_pair_kernel<<<(unsigned)grid, kAttnThreads, kAttnSmem, stream>>>(*kp);
+    if (kind == 2) attn_wide_kernel<<<(unsigned)grid, kAttnThreads, kWideSmem, stream>>>(*kp);
+    else if (kind == 1) attn_pair_kernel<<<(unsigned)grid, kAttnThreads, kAttnSmem, stream>>>(*kp);
     else attn_kernel<<<(unsigned)grid, kAttnThreads, kAttnSmem, stream>>>(*kp);
     return cudaGetLastError() == cudaSuccess ? 0 : -38;
 }

@@ -741,6 +741,7 @@ __global__ void embed_kernel(ds_embed_desc d) {
 // Gated activations (ds_geglu_desc), one thread per 4 outputs of [rows][I], written in format FMT (operand.cuh):
 //   MODE 0, GEGLU: out = x[:, :I] * gelu(x[:, I:]) on fp32 [rows][2I], exact erf GELU.
 //   MODE 1, quick-GELU: out = x * sigmoid(1.702 x) on fp32 [rows][I] (CLIP MLP activation).
+//   MODE 2, exact GELU: out = gelu(x) on fp32 [rows][I] (open_clip ViT-g-14 MLP activation), the erf form of MODE 0.
 template <int MODE, int FMT>
 __global__ void gate_kernel(ds_geglu_desc d) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -755,11 +756,16 @@ __global__ void gate_kernel(ds_geglu_desc d) {
         const float av[4] = {a.x, a.y, a.z, a.w}, gv[4] = {g.x, g.y, g.z, g.w};
 #pragma unroll
         for (int q = 0; q < 4; ++q) y[q] = av[q] * (0.5f * gv[q] * (1.0f + erff(gv[q] * 0.70710678118654752f)));
-    } else {
+    } else if (MODE == 1) {
         const float4 a = *reinterpret_cast<const float4*>(d.src + idx * 4);
         const float av[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
         for (int q = 0; q < 4; ++q) y[q] = av[q] / (1.0f + expf(-1.702f * av[q]));
+    } else {
+        const float4 a = *reinterpret_cast<const float4*>(d.src + idx * 4);
+        const float av[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) y[q] = 0.5f * av[q] * (1.0f + erff(av[q] * 0.70710678118654752f));
     }
     store_operand<4>(reinterpret_cast<__half*>(d.out), d.rows * d.I, idx * 4, y, d.nplanes, FMT);
 }
@@ -945,7 +951,9 @@ extern "C" int ds_layernorm_launch(const ds_layernorm_desc* d, cudaStream_t stre
 
 OpCheck dsb::geglu_check(const ds_geglu_desc& d) {
     if (d.I % 4) return {-2, "geglu: I"};
+    if (d.mode < 0 || d.mode > 2) return {-2, "geglu: mode"};
     if (d.mode == 1 && d.fmt != 0) return {-2, "geglu: quick-GELU fmt"};
+    if (d.mode == 2 && d.fmt != 0) return {-2, "geglu: GELU fmt"};
     if (d.mode != 1 && d.fmt == 1 && d.nplanes != 2) return {-2, "geglu: f8 planes"};
     return {0, nullptr};
 }
@@ -955,6 +963,8 @@ extern "C" int ds_geglu_launch(const ds_geglu_desc* d, cudaStream_t stream) {
     const unsigned blocks = (unsigned)((d->rows * (d->I / 4) + 255) / 256);
     if (d->mode == 1) {
         gate_kernel<1, 0><<<blocks, 256, 0, stream>>>(*d);
+    } else if (d->mode == 2) {
+        gate_kernel<2, 0><<<blocks, 256, 0, stream>>>(*d);
     } else if (d->fmt == 1) {
         gate_kernel<0, 1><<<blocks, 256, 0, stream>>>(*d);
     } else {

@@ -106,6 +106,8 @@ static void visit_ptrs(ds_plan_op& op, F f) {
         case DS_OP_IMG_INPUT: { auto& d = op.u.img_input; P(d.src); P(d.out); break; }
         case DS_OP_IM2COL: { auto& d = op.u.im2col; P(d.src); P(d.out); break; }
         case DS_OP_POOL: { auto& d = op.u.pool; P(d.src); P(d.out_f32); P(d.out_h16); break; }
+        case DS_OP_CLIP_INPUT: { auto& d = op.u.clip_input; P(d.src); P(d.tab); P(d.out); break; }
+        case DS_OP_CLIP_HEAD: { auto& d = op.u.clip_head; P(d.src); P(d.src2); P(d.ids); P(d.out); break; }
         default: break;
     }
 #undef P
@@ -131,6 +133,8 @@ static dsb::OpCheck check_op(const ds_plan_op& op) {
         case DS_OP_IMG_INPUT: return dsb::img_input_check(op.u.img_input);
         case DS_OP_IM2COL: return dsb::im2col_check(op.u.im2col);
         case DS_OP_POOL: return dsb::pool_check(op.u.pool);
+        case DS_OP_CLIP_INPUT: return dsb::clip_input_check(op.u.clip_input);
+        case DS_OP_CLIP_HEAD: return dsb::clip_head_check(op.u.clip_head);
         case DS_OP_SOFTMAX: case DS_OP_POSEMB: case DS_OP_CHANMEAN: case DS_OP_MEMSET: return {0, nullptr};
         default: return {-100, "unknown op type"};
     }
@@ -159,6 +163,8 @@ static int launch_op(const ds_plan_op& op, const unsigned char* gemm_kp, cudaStr
         case DS_OP_IMG_INPUT: return ds_img_input_launch(&op.u.img_input, s);
         case DS_OP_IM2COL: return ds_im2col_launch(&op.u.im2col, s);
         case DS_OP_POOL: return ds_pool_launch(&op.u.pool, s);
+        case DS_OP_CLIP_INPUT: return ds_clip_input_launch(&op.u.clip_input, s);
+        case DS_OP_CLIP_HEAD: return ds_clip_head_launch(&op.u.clip_head, s);
         case DS_OP_ATTN:
             if (gemm_kp) return dsb::attn_run(reinterpret_cast<const dsb::AttnKernelParams*>(gemm_kp), s);
             return ds_attn_launch(&op.u.attn, s);
@@ -515,6 +521,8 @@ size_t ds_sizeof(int which) {
         case DS_OP_IMG_INPUT: return sizeof(ds_img_input_desc);
         case DS_OP_IM2COL: return sizeof(ds_im2col_desc);
         case DS_OP_POOL: return sizeof(ds_pool_desc);
+        case DS_OP_CLIP_INPUT: return sizeof(ds_clip_input_desc);
+        case DS_OP_CLIP_HEAD: return sizeof(ds_clip_head_desc);
         default: return 0;
     }
 }

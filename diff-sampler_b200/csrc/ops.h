@@ -171,20 +171,21 @@ typedef struct ds_gn_finalize_desc {
     int32_t pad1;
 } ds_gn_finalize_desc;
 
-// Fused softmax attention, head dim padded to 64 (attention.cu): out[b][l][h*64 + c] = sum_k softmax_k(scale * q_l . k_k) v_k[c].
+// Fused softmax attention (attention.cu): out[b][l][h*hd + c] = sum_k softmax_k(scale * q_l . k_k) v_k[c], hd = the head width (pad0).
 // All operands are fp16 hi/lo planes, plane p of a [B]-batched tensor at batch index p*B + b.
 // Reference: networks_edm.py:105-118, :174-178; ldm/modules/attention.py:152-196.
 typedef struct ds_attn_desc {
-    const void* q;          // [2][B][L][q_pitch]; head h reads channels q_c0 + h*64 ..
-    const void* k;          // [2][B][Lk][k_pitch]; head h reads channels k_c0 + h*64 ..
-    const void* vt;         // [2][B][nh*64][vt_pitch]: V transposed, keys contiguous (Lk <= vt_pitch valid)
+    const void* q;          // [2][B][L][q_pitch]; head h reads channels q_c0 + h*hd ..
+    const void* k;          // [2][B][Lk][k_pitch]; head h reads channels k_c0 + h*hd ..
+    const void* vt;         // [2][B][nh*hd][vt_pitch]: V transposed, keys contiguous (Lk <= vt_pitch valid)
     void* out;              // [2][B][L][o_pitch]
     int32_t B, nh, L, Lk;
     int32_t q_pitch, q_c0, k_pitch, k_c0, vt_pitch, o_pitch;
     int32_t nplanes;        // must be 2
     float scale;            // > 0
     int32_t causal;         // 1: query l attends to keys <= l only (CLIP text encoder; L == Lk)
-    int32_t pad0;           // head width: 0 or 64, or 32 (heads in pairs: nh even; q/k/out channels and V^T rows at nh*32)
+    int32_t pad0;           // head width hd: 0 or 64; 32 (heads in pairs: nh even; q/k/out channels and V^T rows at nh*32); or 72 .. 128, a
+                            // multiple of 8 (attn_wide_kernel: unpadded heads, no causal mask)
 } ds_attn_desc;
 
 // Row softmax: P = softmax(S) over the last dim, fp32 in, fp16 hi/lo planes out. Reference: networks_edm.py:108.
@@ -271,7 +272,8 @@ typedef struct ds_geglu_desc {
     int32_t I;
     int32_t nplanes;
     int32_t fmt;            // as ds_layernorm_desc.fmt (0 or 1)
-    int32_t mode;           // 0: GEGLU (above).  1: quick-GELU, out = x * sigmoid(1.702 x) on fp32 [rows][I] (CLIP MLP, modeling_clip.py quick_gelu)
+    int32_t mode;           // 0: GEGLU (above).  1: quick-GELU, out = x * sigmoid(1.702 x) on fp32 [rows][I] (CLIP MLP, modeling_clip.py quick_gelu).
+                            // 2: exact erf GELU, out = gelu(x) on fp32 [rows][I] (open_clip ViT-g-14 MLP, nn.GELU()).  Modes 1 and 2 take fmt 0 only.
 } ds_geglu_desc;
 
 // Token + position embedding (CLIPTextEmbeddings.forward): out[row][c] = tok[ids[row]][c] + pos[row % T][c], fp32.
@@ -463,6 +465,47 @@ typedef struct ds_pool_desc {
     int32_t pad0;
 } ds_pool_desc;
 
+// ---------------------------------------------------------------------------------------------
+// CLIP score (clip.cu; open_clip ViT-g-14 as DESIGN.md 4.11 states it).  The towers run on the GEMM, LayerNorm, GELU and attention ops;
+// these two ops are the image preprocessing and the pooled heads.
+//
+// Image input: uint8 images (element (n, c, y, x) at n*sn + c*sc + y*sy + x*sx) -> Pillow's antialiased bicubic resize, horizontal pass
+// then vertical, each pass accumulating uint8 samples times 22-bit fixed-point weights in int32 from 2^21 and clamping (v >> 22) to
+// uint8 -> the S x S centre crop -> (v / 255 - mean[c]) / std[c] in fp32, as fp32 NHWC [B][S][S][3].  The tables are computed on the
+// host in double (openclip_plan.bicubic_tables), indexed by OUTPUT (crop) row / column, int32:
+//   y0[S] ny[S] x0[S] nx[S] wy[S][ky] wx[S][kx]
+// output row i reads source rows y0[i] .. y0[i] + ny[i] - 1 with weights wy[i][0 ..], output column j source columns x0[j] .. with wx[j].
+typedef struct ds_clip_input_desc {
+    const unsigned char* src;
+    const int32_t* tab;
+    float* out;
+    int64_t sn, sc, sy, sx;     // element strides of src
+    int32_t B, H, W, S;
+    int32_t ky, kx;             // taps per row of wy / wx
+    float mean[3];
+    float std[3];
+} ds_clip_input_desc;
+
+// Pooled heads, one CTA per sample n:
+//   GATHER: out[n * out_stride + c] = src[n * src_stride + r * C + c], c < C, with r = argmax_t ids[n * T + t] (the first maximum, the
+//           EOT token of open_clip's text tower) or, ids == NULL, r = row (the class token of the image tower; with src_stride = 0 a
+//           weight row broadcast to every sample);
+//   L2NORM: out[n][c] = src[n][c] / max(||src[n]||, 1e-12)  (sums of squares in fp64);
+//   SCORE:  out[n] = scale * sum_c src[n][c] * src2[n][c]   (fp64 sum).
+enum { DS_CLIP_GATHER = 0, DS_CLIP_L2NORM = 1, DS_CLIP_SCORE = 2 };
+typedef struct ds_clip_head_desc {
+    const float* src;
+    const float* src2;
+    const int32_t* ids;
+    float* out;
+    int64_t src_stride, out_stride;
+    int32_t B, C, T, row;
+    int32_t mode;
+    float scale;
+} ds_clip_head_desc;
+
+int ds_clip_input_launch(const ds_clip_input_desc* d, cudaStream_t stream);
+int ds_clip_head_launch(const ds_clip_head_desc* d, cudaStream_t stream);
 int ds_img_input_launch(const ds_img_input_desc* d, cudaStream_t stream);
 int ds_im2col_launch(const ds_im2col_desc* d, cudaStream_t stream);
 int ds_pool_launch(const ds_pool_desc* d, cudaStream_t stream);
@@ -497,7 +540,8 @@ int ds_embed_launch(const ds_embed_desc* d, cudaStream_t stream);
 enum { DS_OP_GEMM = 1, DS_OP_GN_STATS = 2, DS_OP_GN_APPLY = 3, DS_OP_SOFTMAX = 4, DS_OP_POSEMB = 5, DS_OP_LINEAR = 6,
        DS_OP_PREP_INPUT = 7, DS_OP_CHANMEAN = 8, DS_OP_MEMSET = 9, DS_OP_LAYERNORM = 10, DS_OP_GEGLU = 11,
        DS_OP_GN_FINALIZE = 12, DS_OP_ATTN = 13, DS_OP_EMBED = 14, DS_OP_OPT_PREP = 15, DS_OP_OPT_SOFTMAX = 16,
-       DS_OP_OPT_REDUCE = 17, DS_OP_OPT_KNN = 18, DS_OP_IMG_INPUT = 19, DS_OP_IM2COL = 20, DS_OP_POOL = 21 };
+       DS_OP_OPT_REDUCE = 17, DS_OP_OPT_KNN = 18, DS_OP_IMG_INPUT = 19, DS_OP_IM2COL = 20, DS_OP_POOL = 21,
+       DS_OP_CLIP_INPUT = 22, DS_OP_CLIP_HEAD = 23 };
 enum { DS_IO_X = 0, DS_IO_D = 1, DS_IO_SIGMA = 2, DS_IO_LABELS = 3, DS_IO_BOTTLENECK = 4, DS_IO_CTX = 5, DS_IO_COUNT = 6 };
 
 typedef struct ds_memset_desc {
@@ -530,6 +574,8 @@ typedef struct ds_plan_op {
         ds_img_input_desc img_input;
         ds_im2col_desc im2col;
         ds_pool_desc pool;
+        ds_clip_input_desc clip_input;
+        ds_clip_head_desc clip_head;
     } u;
 } ds_plan_op;
 
@@ -561,5 +607,7 @@ OpCheck opt_knn_check(const ds_opt_knn_desc& d);
 OpCheck img_input_check(const ds_img_input_desc& d);
 OpCheck im2col_check(const ds_im2col_desc& d);
 OpCheck pool_check(const ds_pool_desc& d);
+OpCheck clip_input_check(const ds_clip_input_desc& d);
+OpCheck clip_head_check(const ds_clip_head_desc& d);
 }  // namespace dsb
 #endif

@@ -68,6 +68,38 @@ class FeatureStats:
         return mu.cpu().numpy(), sigma.cpu().numpy()
 
 
+class ScoreStats:
+    """Running sum and count of per-image scores (the CLIP score, clip_score.py:89-93: per rank `avg += score.sum()`, then / N over
+    all images), float64, with the same all-reduce as FeatureStats."""
+
+    def __init__(self):
+        self.total = None
+        self.n = 0
+
+    def append(self, scores):
+        """scores: [B] per-image scores (B200OpenCLIP.score)."""
+        s = scores.to(torch.float64).sum()
+        self.total = s if self.total is None else self.total + s
+        self.n += scores.shape[0]
+        return self
+
+    def reduce(self):
+        """Grand totals over all ranks.  No-op without an initialised process group."""
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            dev = self.total.device if self.total is not None else ('cuda' if dist.get_backend() == 'nccl' else 'cpu')
+            t = torch.stack([torch.as_tensor(0.0 if self.total is None else self.total, dtype=torch.float64, device=dev),
+                             torch.tensor(float(self.n), dtype=torch.float64, device=dev)])
+            dist.all_reduce(t)
+            self.total, self.n = t[0], int(t[1].item())
+        return self
+
+    def mean(self):
+        """The mean score over every image appended (on all ranks, after reduce())."""
+        if self.n < 1:
+            raise ValueError('no scores appended')
+        return float(self.total) / self.n
+
+
 def frechet_distance(mu, sigma, mu_ref, sigma_ref):
     """fid.py:83-87 calculate_fid_from_inception_stats."""
     import scipy.linalg

@@ -294,14 +294,15 @@ class PlanBuilder:
     def attention(self, fused, q, k, out, nh, L, Lk, d, scale, vt_pitch, causal=0, s_pitch=None, pairs=False):
         """softmax(scale Q K^T) V for nh heads of width d over the B batch entries: L queries, Lk keys, V^T in 'vt' (rows of vt_pitch
         keys), O into the fp16 planes `out` [B][L][nh d].  q == k: one [q heads | k heads] buffer of pitch 2 nh d, else two of nh d.
-        fused: the fused kernel (csrc/attention.cu, 64-wide heads, or pairs=True: 32-wide heads two per CTA, nh even); otherwise QK^T into 'S' (rows of s_pitch, default Lk), the row
+        fused: the fused kernel (csrc/attention.cu, 64-wide heads, or pairs=True: 32-wide heads two per CTA, nh even, or d in 72 .. 128:
+        unpadded wide heads); otherwise QK^T into 'S' (rows of s_pitch, default Lk), the row
         softmax into 'P' (rows of vt_pitch) and the P.V GEMM."""
         B, C = self.B, nh * d
         qp, kc0 = (2 * C, C) if q == k else (C, 0)
         if fused:
             self.emit(lambda R: S.AttnDesc(q=R(q), k=R(k), vt=R('vt'), out=R(out), B=B, nh=nh, L=L, Lk=Lk, q_pitch=qp, q_c0=0,
                                            k_pitch=qp, k_c0=kc0, vt_pitch=vt_pitch, o_pitch=C, nplanes=NPL, scale=scale, causal=causal,
-                                           pad0=32 if pairs else 0))
+                                           pad0=32 if pairs else (d if d > 64 else 0)))
             return
         sp = s_pitch or Lk
         self.need('S', B * nh * L * sp * F4)
