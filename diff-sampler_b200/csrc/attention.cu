@@ -400,8 +400,9 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_pair_kernel(const __grid
 // TMA zero-fills channels (V^T rows) hd .. 127, so no GEMM pads its output to 128 and the zero channels add nothing to S or O.  S takes
 // ceil(hd / 16) k16 steps per pass; O is two m64n64k16 accumulators (d-rows 0..63, 64..127), of which the store keeps columns < hd.
 // Q is 64 KB and a K + V^T stage 64 KB, so the ring has 2 stages.  O[64] accumulates in the wgmma itself (alpha-scaled first, no
-// per-block accumulator as in attn_kernel): that keeps S, P and O within the 168 registers of a 384-thread CTA without a stack frame;
-// with at most a few hundred keys the tensor cores' accumulation error stays at the level of one key block.
+// per-block accumulator as in attn_kernel): that keeps S, P and O within the 168 registers of a 384-thread CTA without a stack frame.
+// The tensor cores' accumulation error then grows with the key count: measured on an H100 80GB HBM3, 3.6e-6 of max |O| at 257 keys,
+// 7.0e-6 at 730 and 8.9e-6 at 1025 with values of mean 1 (tests/test_gpu_openclip.py), against 2e-5 allowed.
 static constexpr int kWideStages = 2;
 static constexpr int kWideQBytes = 4 * 16384;      // Q hi, lo: 2 channel blocks x 128 rows x 64 fp16 each
 static constexpr int kWideKBytes = 4 * 8192;       // K hi, lo: 2 channel blocks x 64 keys x 64

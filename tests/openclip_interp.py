@@ -39,7 +39,9 @@ def clip_input(mem, d):
     v = clip8((1 << 21) + (h[:, :, iy, :] * ky_[:, :, None]).sum(3))              # [B][3][Sz][Sz]
     mean = torch.tensor(list(d.mean), dtype=torch.float32, device=mem.device)[:, None, None]
     std = torch.tensor(list(d.std), dtype=torch.float32, device=mem.device)[:, None, None]
-    y = (v.float() / 255.0 - mean) / std
+    # ToTensor's x / 255 as a true fp32 division on every device: CUDA tensors divide by a CPU scalar as a multiplication by its
+    # rounded reciprocal, one ulp off for half of the 256 values
+    y = (v.float() / torch.tensor(255.0, device=mem.device) - mean) / std
     mem.view(d.out, torch.float32, B * Sz * Sz * 3)[:] = y.permute(0, 2, 3, 1).reshape(-1)
 
 

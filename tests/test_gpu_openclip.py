@@ -58,6 +58,128 @@ def test_wide_attention_against_float64(nh, hd, L, Lk):
     assert err < 2e-5
 
 
+# ------------------------------------------------------------------------------------------ the wide kernel at its edges
+WIDE_HDS = list(range(72, 129, 8))            # every width attn_check accepts: the second 64-channel box holds 8 .. 64 channels
+WIDE_LKS = [1, 63, 64, 65, 128, 129, 257, 730, 1025]
+WIDE_LS = [1, 127, 128, 129, 257]
+GUARD = 4096                                  # fp16 elements of NaN before and after every buffer
+
+
+def _guarded(n):
+    """A NaN-filled fp16 buffer with GUARD elements on both sides, and its inner n elements."""
+    buf = torch.full((2 * GUARD + n,), float('nan'), dtype=torch.float16, device=DEV)
+    return buf, buf[GUARD:GUARD + n]
+
+
+def _wide_case(nh, hd, L, Lk, B=2, layout='qk', v_mean=0.0, late=False, seed=0):
+    """attn_wide_kernel against float64 softmax attention on the same fp16 hi + lo operands.  Every byte the kernel must not read or
+    write is NaN: the Q / K channels outside the heads' window of each row, the V^T columns Lk .. vt_pitch, the output channels
+    nh hd .. o_pitch, and a guard before and after each buffer.  A read of any of them would make an output NaN; the output
+    sentinels must still be NaN afterwards, the inputs bit for bit unchanged.  Returns the error / max |O|.
+
+    layout 'qk': the plan's [q | k] rows (L == Lk, q_pitch = k_pitch = 2 C, k_c0 = C, vt_pitch = Lk rounded up to 8, o_pitch = C);
+    'sep': Q and K in buffers of their own with q_c0 = 16, k_c0 = 40, pitches C + 40 and C + 48, 8 spare V^T columns, o_pitch C + 16.
+    late: every third query row gets its maximum logit, about 30 above the rest, from the last key alone, so the last key block
+    rescales O (alpha ~ e^-30) after all the others have been accumulated."""
+    C, scale = nh * hd, hd ** -0.5
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    q = torch.randn(B, L, nh, hd, generator=g, device=DEV)
+    k = torch.randn(B, Lk, nh, hd, generator=g, device=DEV)
+    v = torch.randn(B, Lk, nh, hd, generator=g, device=DEV) + v_mean
+    if late:
+        u = torch.randn(nh, hd, generator=g, device=DEV)
+        u /= u.norm(dim=1, keepdim=True)
+        q[:, ::3] = 3 * u
+        k[:, Lk - 1] = 10 / scale * u                                    # logit scale * 3 * 10 / scale = 30
+    if layout == 'qk':
+        assert L == Lk
+        q_c0, k_c0, qp, kp, vp, op = 0, C, 2 * C, 2 * C, -(-Lk // 8) * 8, C
+    else:
+        q_c0, k_c0, qp, kp, vp, op = 16, 40, C + 40, C + 48, -(-Lk // 8) * 8 + 8, C + 16
+
+    def operand(rows, pitch, c0, x):                                      # fp32 [B][rows][pitch], NaN outside the heads
+        t = torch.full((B, rows, pitch), float('nan'), device=DEV)
+        t[:, :, c0:c0 + C] = x.reshape(B, rows, C)
+        return t
+    qf = operand(L, qp, q_c0, q)
+    kf = operand(Lk, kp, k_c0, k)
+    if layout == 'qk':
+        qf[:, :, k_c0:k_c0 + C] = kf[:, :, k_c0:k_c0 + C]
+        kf = None
+    vf = torch.full((B, C, vp), float('nan'), device=DEV)
+    vf[:, :, :Lk] = v.permute(0, 2, 3, 1).reshape(B, C, Lk)
+    bufs = []
+
+    def place(x):                                                         # fp16 planes [2][..] inside a guarded buffer
+        hi, lo = _split(x)
+        buf, inner = _guarded(2 * x.numel())
+        inner.view(2, -1).copy_(torch.stack([hi, lo]).reshape(2, -1))
+        bufs.append((buf, buf.clone()))
+        return inner, hi.double() + lo.double()
+    qd, q64 = place(qf)
+    kd, k64 = place(kf) if kf is not None else (qd, q64)
+    vd, v64 = place(vf)
+    obuf, od = _guarded(2 * B * L * op)
+    _lib.op_launch(S.AttnDesc(q=qd.data_ptr(), k=kd.data_ptr(), vt=vd.data_ptr(), out=od.data_ptr(), B=B, nh=nh, L=L, Lk=Lk, q_pitch=qp,
+                              q_c0=q_c0, k_pitch=kp, k_c0=k_c0, vt_pitch=vp, o_pitch=op, nplanes=2, scale=scale, causal=0, pad0=hd))
+    torch.cuda.synchronize()
+    for buf, before in bufs:
+        assert torch.equal(buf.view(torch.int16), before.view(torch.int16)), 'an input buffer changed'
+    out = od.view(2, B, L, op)
+    assert torch.isfinite(out[..., :C]).all(), 'non-finite output: a NaN sentinel was read, or a row was left unwritten'
+    assert torch.isnan(out[..., C:]).all() and torch.isnan(obuf[:GUARD]).all() and torch.isnan(obuf[GUARD + od.numel():]).all(), \
+        'a store outside the output rows'
+    got = (out[0].double() + out[1].double())[..., :C].reshape(B, L, nh, hd).transpose(1, 2)
+    qs = q64[:, :, q_c0:q_c0 + C].reshape(B, L, nh, hd).transpose(1, 2)
+    ks = k64[:, :, k_c0:k_c0 + C].reshape(B, Lk, nh, hd).transpose(1, 2)
+    vs = v64[:, :, :Lk].reshape(B, nh, hd, Lk).transpose(2, 3)
+    s = scale * qs @ ks.transpose(2, 3)
+    want = torch.softmax(s, dim=3) @ vs
+    if late:                                                              # the construction did what it claims
+        top = s[:, :, ::3].topk(2, dim=3)
+        assert (top.indices[..., 0] == Lk - 1).all() and (top.values[..., 0] - top.values[..., 1]).min() > 25
+    err = ((got - want).abs().max() / want.abs().max()).item()
+    print(f'wide attention hd {hd:3d} L {L:4d} Lk {Lk:4d} nh {nh} B {B} {layout}{f" v_mean {v_mean}" if v_mean else ""}'
+          f'{" late max" if late else ""}: {err:.2e} of max |O|')
+    return err
+
+
+# Error / max |O| measured on an H100 80GB HBM3 (700 W power limit), worst over the head widths: 3.6e-6 up to 257 keys, 7.0e-6 at 730
+# and 8.9e-6 at 1025 keys with values of mean 1; 3.0e-6 with the late maximum, 3.0e-6 over 3072 CTAs.  O accumulates inside the wgmma
+# across all key blocks, so the error grows about linearly with the key count; at that rate it would reach this bound near 2300 keys.
+WIDE_TOL = 2e-5
+
+
+@pytest.mark.parametrize('Lk', WIDE_LKS)
+@pytest.mark.parametrize('hd', WIDE_HDS)
+def test_wide_attention_widths_and_key_counts(hd, Lk):
+    """Self-attention in the plan's layout at every accepted head width and at key counts of one key, a partial block, an exact
+    block, one key into the next block, and the two plan sizes (257, 730 tokens) and one past them; values of mean 1 at 730 and
+    1025 keys, where O's error grows with the key count."""
+    assert _wide_case(4, hd, Lk, Lk, v_mean=1.0 if Lk >= 730 else 0.0, seed=hd + Lk) < WIDE_TOL
+
+
+@pytest.mark.parametrize('Lk', [1, 65, 730])
+@pytest.mark.parametrize('L', WIDE_LS)
+def test_wide_attention_cross_shapes_and_pitches(L, Lk):
+    """Cross-attention (L != Lk apart from 1 x 1) over separate Q and K buffers with channel offsets, unequal pitches, spare V^T
+    columns and an output pitch wider than the heads; the head width cycles through the accepted widths."""
+    hd = WIDE_HDS[(WIDE_LS.index(L) * 3 + [1, 65, 730].index(Lk)) % len(WIDE_HDS)]
+    assert _wide_case(3, hd, L, Lk, B=3, layout='sep', v_mean=0.5, seed=L + Lk) < WIDE_TOL
+
+
+@pytest.mark.parametrize('hd,L,Lk,layout', [(72, 129, 129, 'qk'), (88, 257, 257, 'qk'), (80, 730, 730, 'qk'), (128, 1025, 1025, 'qk'),
+                                             (104, 300, 1025, 'sep'), (120, 129, 730, 'sep')])
+def test_wide_attention_late_maximum(hd, L, Lk, layout):
+    """Rows whose maximum logit first appears in the last, partial key block, about 30 above all the others."""
+    assert _wide_case(4, hd, L, Lk, layout=layout, v_mean=1.0, late=True, seed=hd) < WIDE_TOL
+
+
+def test_wide_attention_many_waves():
+    """Batch 64 x 16 heads of 88 x 3 query tiles: 3072 CTAs (the max_batch chunk of ViT-g-14), many waves over the SMs."""
+    assert _wide_case(16, 88, 257, 257, B=64, seed=1) < WIDE_TOL
+
+
 @pytest.mark.parametrize('H,W', [(512, 512), (256, 256), (64, 64), (512, 768), (768, 512), (224, 300)])
 @pytest.mark.parametrize('nhwc', [False, True])
 def test_image_input_is_bit_identical_to_the_restatement(H, W, nhwc):
