@@ -6,12 +6,15 @@ P = C.c_uint64      # pointer fields: absolute device address or a reference (sp
 I32 = C.c_int32
 I64 = C.c_int64
 F32 = C.c_float
+F64 = C.c_double
 
 DS_OP_GEMM, DS_OP_GN_STATS, DS_OP_GN_APPLY, DS_OP_SOFTMAX, DS_OP_POSEMB, DS_OP_LINEAR = 1, 2, 3, 4, 5, 6
 DS_OP_PREP_INPUT, DS_OP_CHANMEAN, DS_OP_MEMSET, DS_OP_LAYERNORM, DS_OP_GEGLU, DS_OP_GN_FINALIZE, DS_OP_ATTN, DS_OP_EMBED = 7, 8, 9, 10, 11, 12, 13, 14
 DS_OP_OPT_PREP, DS_OP_OPT_SOFTMAX, DS_OP_OPT_REDUCE, DS_OP_OPT_KNN = 15, 16, 17, 18
 DS_OP_IMG_INPUT, DS_OP_IM2COL, DS_OP_POOL = 19, 20, 21
 DS_OP_CLIP_INPUT, DS_OP_CLIP_HEAD = 22, 23
+DS_OP_PRDC_KTH, DS_OP_PRDC_COUNT = 24, 25
+DS_PRDC_KMAX, DS_PRDC_LIST = 63, 1024     # csrc/ops.h: largest nearest_k of prdc_kth, length of its rescoring list
 DS_CLIP_GATHER, DS_CLIP_L2NORM, DS_CLIP_SCORE = 0, 1, 2
 DS_POOL_MAX, DS_POOL_AVG, DS_POOL_MEAN = 0, 1, 2
 DS_IO_X, DS_IO_D, DS_IO_SIGMA, DS_IO_LABELS, DS_IO_BOTTLENECK, DS_IO_CTX, DS_IO_COUNT = 0, 1, 2, 3, 4, 5, 6
@@ -151,6 +154,17 @@ class ClipHeadDesc(C.Structure):
                 ('row', I32), ('mode', I32), ('scale', F32)]
 
 
+class PrdcKthDesc(C.Structure):
+    _fields_ = [('part', P), ('q', P), ('t', P), ('qn2', P), ('tn2', P), ('rad', P), ('rad2', P), ('nres', P), ('ldp', I64),
+                ('B', I32), ('N', I32), ('D', I32), ('nslice', I32), ('k', I32), ('pad0', I32), ('sq', F64), ('st', F64)]
+
+
+class PrdcCountDesc(C.Structure):
+    _fields_ = [('part', P), ('q', P), ('t', P), ('qn2', P), ('tn2', P), ('tau', P), ('tau2', P), ('rho', P), ('rho2', P), ('cnt_t', P),
+                ('cnt_own', P), ('realism', P), ('nres', P), ('ldp', I64), ('B', I32), ('N', I32), ('D', I32), ('nslice', I32),
+                ('sq', F64), ('st', F64), ('med', F64)]
+
+
 class MemsetDesc(C.Structure):
     _fields_ = [('ptr', P), ('bytes', I64)]
 
@@ -161,7 +175,7 @@ class _OpUnion(C.Union):
                 ('memset', MemsetDesc), ('layernorm', LayernormDesc), ('geglu', GegluDesc), ('gn_finalize', GnFinalizeDesc), ('attn', AttnDesc),
                 ('embed', EmbedDesc), ('opt_prep', OptPrepDesc), ('opt_softmax', OptSoftmaxDesc), ('opt_reduce', OptReduceDesc),
                 ('opt_knn', OptKnnDesc), ('img_input', ImgInputDesc), ('im2col', Im2colDesc), ('pool', PoolDesc),
-                ('clip_input', ClipInputDesc), ('clip_head', ClipHeadDesc)]
+                ('clip_input', ClipInputDesc), ('clip_head', ClipHeadDesc), ('prdc_kth', PrdcKthDesc), ('prdc_count', PrdcCountDesc)]
 
 
 class PlanOp(C.Structure):
@@ -174,7 +188,7 @@ SIZEOF_CHECKS = {
     DS_OP_MEMSET: MemsetDesc, DS_OP_LAYERNORM: LayernormDesc, DS_OP_GEGLU: GegluDesc, DS_OP_GN_FINALIZE: GnFinalizeDesc, DS_OP_ATTN: AttnDesc,
     DS_OP_EMBED: EmbedDesc, DS_OP_OPT_PREP: OptPrepDesc, DS_OP_OPT_SOFTMAX: OptSoftmaxDesc, DS_OP_OPT_REDUCE: OptReduceDesc,
     DS_OP_OPT_KNN: OptKnnDesc, DS_OP_IMG_INPUT: ImgInputDesc, DS_OP_IM2COL: Im2colDesc, DS_OP_POOL: PoolDesc,
-    DS_OP_CLIP_INPUT: ClipInputDesc, DS_OP_CLIP_HEAD: ClipHeadDesc,
+    DS_OP_CLIP_INPUT: ClipInputDesc, DS_OP_CLIP_HEAD: ClipHeadDesc, DS_OP_PRDC_KTH: PrdcKthDesc, DS_OP_PRDC_COUNT: PrdcCountDesc,
 }
 
 # Union member of each op type of the network plans (plan.py, ldm_plan.py, vae_plan.py, clip_plan.py) ...
@@ -189,10 +203,12 @@ OPT_UNION_FIELD = {DS_OP_OPT_PREP: 'opt_prep', DS_OP_OPT_SOFTMAX: 'opt_softmax',
 INCEPTION_UNION_FIELD = {DS_OP_IMG_INPUT: 'img_input', DS_OP_IM2COL: 'im2col', DS_OP_POOL: 'pool'}
 # ... and of the ops only the CLIP-score towers (openclip_plan.py) add.
 OPENCLIP_UNION_FIELD = {DS_OP_CLIP_INPUT: 'clip_input', DS_OP_CLIP_HEAD: 'clip_head'}
-ALL_UNION_FIELD = {**UNION_FIELD, **OPT_UNION_FIELD, **INCEPTION_UNION_FIELD, **OPENCLIP_UNION_FIELD}
+# ... and of the ops only the PRDC plans (prdc.py) add.
+PRDC_UNION_FIELD = {DS_OP_PRDC_KTH: 'prdc_kth', DS_OP_PRDC_COUNT: 'prdc_count'}
+ALL_UNION_FIELD = {**UNION_FIELD, **OPT_UNION_FIELD, **INCEPTION_UNION_FIELD, **OPENCLIP_UNION_FIELD, **PRDC_UNION_FIELD}
 OP_TYPE_OF = {GemmDesc: DS_OP_GEMM, GnStatsDesc: DS_OP_GN_STATS, GnApplyDesc: DS_OP_GN_APPLY, SoftmaxDesc: DS_OP_SOFTMAX,
               PosembDesc: DS_OP_POSEMB, LinearDesc: DS_OP_LINEAR, PrepInputDesc: DS_OP_PREP_INPUT, ChanmeanDesc: DS_OP_CHANMEAN,
               MemsetDesc: DS_OP_MEMSET, LayernormDesc: DS_OP_LAYERNORM, GegluDesc: DS_OP_GEGLU, GnFinalizeDesc: DS_OP_GN_FINALIZE, AttnDesc: DS_OP_ATTN,
               EmbedDesc: DS_OP_EMBED, OptPrepDesc: DS_OP_OPT_PREP, OptSoftmaxDesc: DS_OP_OPT_SOFTMAX, OptReduceDesc: DS_OP_OPT_REDUCE,
               OptKnnDesc: DS_OP_OPT_KNN, ImgInputDesc: DS_OP_IMG_INPUT, Im2colDesc: DS_OP_IM2COL, PoolDesc: DS_OP_POOL,
-              ClipInputDesc: DS_OP_CLIP_INPUT, ClipHeadDesc: DS_OP_CLIP_HEAD}
+              ClipInputDesc: DS_OP_CLIP_INPUT, ClipHeadDesc: DS_OP_CLIP_HEAD, PrdcKthDesc: DS_OP_PRDC_KTH, PrdcCountDesc: DS_OP_PRDC_COUNT}

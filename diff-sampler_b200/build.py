@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libdiffsampler_b200.so')
-SOURCES = ['gemm_tc.cu', 'attention.cu', 'elementwise.cu', 'solver.cu', 'optimal.cu', 'inception.cu', 'clip.cu', 'engine.cu']
+SOURCES = ['gemm_tc.cu', 'attention.cu', 'elementwise.cu', 'solver.cu', 'optimal.cu', 'inception.cu', 'clip.cu', 'prdc.cu', 'engine.cu']
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
                      '-Xcompiler', '-fPIC', '--use_fast_math' if False else '-DDSB_NO_FAST_MATH']

@@ -108,6 +108,17 @@ static void visit_ptrs(ds_plan_op& op, F f) {
         case DS_OP_POOL: { auto& d = op.u.pool; P(d.src); P(d.out_f32); P(d.out_h16); break; }
         case DS_OP_CLIP_INPUT: { auto& d = op.u.clip_input; P(d.src); P(d.tab); P(d.out); break; }
         case DS_OP_CLIP_HEAD: { auto& d = op.u.clip_head; P(d.src); P(d.src2); P(d.ids); P(d.out); break; }
+        case DS_OP_PRDC_KTH: {
+            auto& d = op.u.prdc_kth;
+            P(d.part); P(d.q); P(d.t); P(d.qn2); P(d.tn2); P(d.rad); P(d.rad2); P(d.nres);
+            break;
+        }
+        case DS_OP_PRDC_COUNT: {
+            auto& d = op.u.prdc_count;
+            P(d.part); P(d.q); P(d.t); P(d.qn2); P(d.tn2); P(d.tau); P(d.tau2); P(d.rho); P(d.rho2); P(d.cnt_t); P(d.cnt_own);
+            P(d.realism); P(d.nres);
+            break;
+        }
         default: break;
     }
 #undef P
@@ -135,6 +146,8 @@ static dsb::OpCheck check_op(const ds_plan_op& op) {
         case DS_OP_POOL: return dsb::pool_check(op.u.pool);
         case DS_OP_CLIP_INPUT: return dsb::clip_input_check(op.u.clip_input);
         case DS_OP_CLIP_HEAD: return dsb::clip_head_check(op.u.clip_head);
+        case DS_OP_PRDC_KTH: return dsb::prdc_kth_check(op.u.prdc_kth);
+        case DS_OP_PRDC_COUNT: return dsb::prdc_count_check(op.u.prdc_count);
         case DS_OP_SOFTMAX: case DS_OP_POSEMB: case DS_OP_CHANMEAN: case DS_OP_MEMSET: return {0, nullptr};
         default: return {-100, "unknown op type"};
     }
@@ -165,6 +178,8 @@ static int launch_op(const ds_plan_op& op, const unsigned char* gemm_kp, cudaStr
         case DS_OP_POOL: return ds_pool_launch(&op.u.pool, s);
         case DS_OP_CLIP_INPUT: return ds_clip_input_launch(&op.u.clip_input, s);
         case DS_OP_CLIP_HEAD: return ds_clip_head_launch(&op.u.clip_head, s);
+        case DS_OP_PRDC_KTH: return ds_prdc_kth_launch(&op.u.prdc_kth, s);
+        case DS_OP_PRDC_COUNT: return ds_prdc_count_launch(&op.u.prdc_count, s);
         case DS_OP_ATTN:
             if (gemm_kp) return dsb::attn_run(reinterpret_cast<const dsb::AttnKernelParams*>(gemm_kp), s);
             return ds_attn_launch(&op.u.attn, s);
@@ -523,6 +538,8 @@ size_t ds_sizeof(int which) {
         case DS_OP_POOL: return sizeof(ds_pool_desc);
         case DS_OP_CLIP_INPUT: return sizeof(ds_clip_input_desc);
         case DS_OP_CLIP_HEAD: return sizeof(ds_clip_head_desc);
+        case DS_OP_PRDC_KTH: return sizeof(ds_prdc_kth_desc);
+        case DS_OP_PRDC_COUNT: return sizeof(ds_prdc_count_desc);
         default: return 0;
     }
 }

@@ -504,6 +504,60 @@ typedef struct ds_clip_head_desc {
     float scale;
 } ds_clip_head_desc;
 
+// ---------------------------------------------------------------------------------------------
+// Precision, recall, density and coverage (prdc.cu; sfd-main/prdc.py as DESIGN.md 4.12 states it).  Every distance product runs on the
+// GEMM kernel (rows mode): part[s][b][i] (s < nslice, row pitch ldp) are the fp32 partials over channel slice s of
+// sq st q_b.t_i, the fp16 hi/lo planes of the query and target rows scaled by the powers of two sq and st.  The rows themselves are kept
+// in float64 (q [B][D], t [N][D]) with their squared norms qn2 / tn2; d2_bi = qn2_b + tn2_i - 2 (sum_s part) / (sq st) approximates
+// ||q_b - t_i||^2 within a per-pair bound (DESIGN.md 4.12).  Pairs the bound cannot decide are recomputed exactly, one warp per pair:
+// float64 differences, squares and sums in a fixed order, then sqrt; comparisons are on those float64 distances.  There is no cap on
+// the number of recomputed pairs; nres[b] (may be NULL) receives how many pairs row b recomputed.
+//
+// prdc_kth: rad[b] = the (k+1)-th smallest ||q_b - t_i|| (the target set is the query's own set, so the self distance 0 counts),
+// rad2[b] its exact squared distance.  Overwrites part slice 0 with d2 (fp32).  k <= DS_PRDC_KMAX.
+enum { DS_PRDC_KMAX = 63, DS_PRDC_LIST = 1024 };
+typedef struct ds_prdc_kth_desc {
+    float* part;
+    const double* q;
+    const double* t;
+    const double* qn2;      // [B]
+    const double* tn2;      // [N]
+    double* rad;            // [B]
+    double* rad2;           // [B]
+    int32_t* nres;          // [B], may be NULL
+    int64_t ldp;
+    int32_t B, N, D, nslice;
+    int32_t k, pad0;
+    double sq, st;          // operand scales (powers of two)
+} ds_prdc_kth_desc;
+
+// prdc_count: for each query row b against targets with radii tau_i (tau2_i their exact squared distances):
+//   cnt_t[b]   = #{i : ||q_b - t_i|| < tau_i};
+//   cnt_own[b] = #{i : ||q_b - t_i|| < rho_b}            (rho / rho2 / cnt_own all set, or all NULL);
+//   realism[b] = max over {i : tau_i < med} of tau_i / ||q_b - t_i||   (may be NULL; x / 0 = inf, 0 / 0 = nan, nan wins).
+typedef struct ds_prdc_count_desc {
+    const float* part;
+    const double* q;
+    const double* t;
+    const double* qn2;
+    const double* tn2;
+    const double* tau;      // [N]
+    const double* tau2;     // [N]
+    const double* rho;      // [B]
+    const double* rho2;     // [B]
+    int32_t* cnt_t;         // [B]
+    int32_t* cnt_own;       // [B]
+    double* realism;        // [B]
+    int32_t* nres;          // [B], may be NULL
+    int64_t ldp;
+    int32_t B, N, D, nslice;
+    double sq, st;
+    double med;
+} ds_prdc_count_desc;
+
+int ds_prdc_kth_launch(const ds_prdc_kth_desc* d, cudaStream_t stream);
+int ds_prdc_count_launch(const ds_prdc_count_desc* d, cudaStream_t stream);
+
 int ds_clip_input_launch(const ds_clip_input_desc* d, cudaStream_t stream);
 int ds_clip_head_launch(const ds_clip_head_desc* d, cudaStream_t stream);
 int ds_img_input_launch(const ds_img_input_desc* d, cudaStream_t stream);
@@ -541,7 +595,7 @@ enum { DS_OP_GEMM = 1, DS_OP_GN_STATS = 2, DS_OP_GN_APPLY = 3, DS_OP_SOFTMAX = 4
        DS_OP_PREP_INPUT = 7, DS_OP_CHANMEAN = 8, DS_OP_MEMSET = 9, DS_OP_LAYERNORM = 10, DS_OP_GEGLU = 11,
        DS_OP_GN_FINALIZE = 12, DS_OP_ATTN = 13, DS_OP_EMBED = 14, DS_OP_OPT_PREP = 15, DS_OP_OPT_SOFTMAX = 16,
        DS_OP_OPT_REDUCE = 17, DS_OP_OPT_KNN = 18, DS_OP_IMG_INPUT = 19, DS_OP_IM2COL = 20, DS_OP_POOL = 21,
-       DS_OP_CLIP_INPUT = 22, DS_OP_CLIP_HEAD = 23 };
+       DS_OP_CLIP_INPUT = 22, DS_OP_CLIP_HEAD = 23, DS_OP_PRDC_KTH = 24, DS_OP_PRDC_COUNT = 25 };
 enum { DS_IO_X = 0, DS_IO_D = 1, DS_IO_SIGMA = 2, DS_IO_LABELS = 3, DS_IO_BOTTLENECK = 4, DS_IO_CTX = 5, DS_IO_COUNT = 6 };
 
 typedef struct ds_memset_desc {
@@ -576,6 +630,8 @@ typedef struct ds_plan_op {
         ds_pool_desc pool;
         ds_clip_input_desc clip_input;
         ds_clip_head_desc clip_head;
+        ds_prdc_kth_desc prdc_kth;
+        ds_prdc_count_desc prdc_count;
     } u;
 } ds_plan_op;
 
@@ -609,5 +665,7 @@ OpCheck im2col_check(const ds_im2col_desc& d);
 OpCheck pool_check(const ds_pool_desc& d);
 OpCheck clip_input_check(const ds_clip_input_desc& d);
 OpCheck clip_head_check(const ds_clip_head_desc& d);
+OpCheck prdc_kth_check(const ds_prdc_kth_desc& d);
+OpCheck prdc_count_check(const ds_prdc_count_desc& d);
 }  // namespace dsb
 #endif
