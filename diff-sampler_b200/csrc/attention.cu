@@ -59,70 +59,160 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
-__global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_constant__ AttnKernelParams p) {
+// Where a CTA works and its shared memory, the same for the three kernels.
+struct AttnCta {
+    uint8_t* smem;              // dynamic shared memory, aligned to 1024 bytes
+    AttnCtl* ctl;
+    int wg;                     // warpgroup: 0 producer, 1 and 2 queries
+    int qt, h, b;               // query tile, head (head pair in attn_pair_kernel), sample
+    int nkv;                    // key blocks the tile reads
+};
+
+// Prologue of every kernel: decodes (query tile, head, sample) from blockIdx.x and counts the key blocks (kCausal: the kernel applies
+// p.causal); thread 0 prefetches the tensor maps and initialises the barriers of a kStages-deep ring in the control block at kOffCtl.
+template <int kStages, int kOffCtl, bool kCausal>
+__device__ __forceinline__ AttnCta attn_prologue(const AttnKernelParams& p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    AttnCtl* ctl = reinterpret_cast<AttnCtl*>(smem + kOffCtl);
-
-    const int wg = threadIdx.x >> 7;
-    const int qt = blockIdx.x % p.q_tiles;
+    AttnCta cta;
+    cta.smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    cta.ctl = reinterpret_cast<AttnCtl*>(cta.smem + kOffCtl);
+    cta.wg = threadIdx.x >> 7;
+    cta.qt = blockIdx.x % p.q_tiles;
     const int z = blockIdx.x / p.q_tiles;
-    const int h = z % p.nh;
-    const int b = z / p.nh;
+    cta.h = z % p.nh;
+    cta.b = z / p.nh;
     // causal: the tile's last query sees keys up to qt * 128 + 127
-    const int lk_eff = p.causal ? min(p.Lk, qt * 128 + 128) : p.Lk;
-    const int nkv = (lk_eff + 63) >> 6;
-
+    const int lk_eff = kCausal && p.causal ? min(p.Lk, cta.qt * 128 + 128) : p.Lk;
+    cta.nkv = (lk_eff + 63) >> 6;
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.tmQ);
         tma_prefetch_desc(&p.tmK);
         tma_prefetch_desc(&p.tmV);
-        mbar_init(&ctl->q_full, 1);
-        for (int s = 0; s < kAttnStages; ++s) {
-            mbar_init(&ctl->kv_full[s], 1);
-            mbar_init(&ctl->kv_empty[s], 2);                              // one arrival per query warpgroup
+        mbar_init(&cta.ctl->q_full, 1);
+        for (int s = 0; s < kStages; ++s) {
+            mbar_init(&cta.ctl->kv_full[s], 1);
+            mbar_init(&cta.ctl->kv_empty[s], 2);                            // one arrival per query warpgroup
         }
         fence_barrier_init();
     }
     __syncthreads();
+    return cta;
+}
 
-    if (wg == 0) {
-        if (threadIdx.x == 0) {
-            mbar_arrive_expect_tx(&ctl->q_full, kQBytes);
-            tma_load_3d(&p.tmQ, &ctl->q_full, smem, p.q_c0 + h * 64, qt * 128, b);
-            tma_load_3d(&p.tmQ, &ctl->q_full, smem + 16384, p.q_c0 + h * 64, qt * 128, p.B + b);
-            for (int j = 0; j < nkv; ++j) {
-                const int s = j % kAttnStages;
-                const uint32_t ph = (j / kAttnStages) & 1;
-                mbar_wait(&ctl->kv_empty[s], ph ^ 1);
-                mbar_arrive_expect_tx(&ctl->kv_full[s], kStageBytes);
-                uint8_t* sk = smem + kOffKV + s * kStageBytes;
-                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk, p.k_c0 + h * 64, j * 64, b);
-                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk + 8192, p.k_c0 + h * 64, j * 64, p.B + b);
-                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes, j * 64, h * 64, b);
-                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes + 8192, j * 64, h * 64, p.B + b);
-            }
+// TMA producer of attn_kernel and attn_pair_kernel (thread 0): the Q tile once, then K_j and V_j^T of the CTA's 64 channels (a head or
+// a head pair) for key blocks 0 .. nkv - 1 into the ring, hi and lo plane each.
+__device__ __forceinline__ void attn_produce(const AttnKernelParams& p, const AttnCta& cta) {
+    mbar_arrive_expect_tx(&cta.ctl->q_full, kQBytes);
+    tma_load_3d(&p.tmQ, &cta.ctl->q_full, cta.smem, p.q_c0 + cta.h * 64, cta.qt * 128, cta.b);
+    tma_load_3d(&p.tmQ, &cta.ctl->q_full, cta.smem + 16384, p.q_c0 + cta.h * 64, cta.qt * 128, p.B + cta.b);
+    for (int j = 0; j < cta.nkv; ++j) {
+        const int s = j % kAttnStages;
+        const uint32_t ph = (j / kAttnStages) & 1;
+        mbar_wait(&cta.ctl->kv_empty[s], ph ^ 1);
+        mbar_arrive_expect_tx(&cta.ctl->kv_full[s], kStageBytes);
+        uint8_t* sk = cta.smem + kOffKV + s * kStageBytes;
+        tma_load_3d(&p.tmK, &cta.ctl->kv_full[s], sk, p.k_c0 + cta.h * 64, j * 64, cta.b);
+        tma_load_3d(&p.tmK, &cta.ctl->kv_full[s], sk + 8192, p.k_c0 + cta.h * 64, j * 64, p.B + cta.b);
+        tma_load_3d(&p.tmV, &cta.ctl->kv_full[s], sk + kKBytes, j * 64, cta.h * 64, cta.b);
+        tma_load_3d(&p.tmV, &cta.ctl->kv_full[s], sk + kKBytes + 8192, j * 64, cta.h * 64, p.B + cta.b);
+    }
+}
+
+// Online softmax of one key block on the thread's S fragment: S[4 g + e] is row r0 + 8 (e >> 1), key 8 g + 2 (lane & 3) + (e & 1) of
+// the block, and column c of row half hr is valid iff c < kv[hr].  Updates the running max m (of scale_log2e * s) and sum l of each row
+// and returns alpha, the factor for what was accumulated before this block, and P = exp2(scale_log2e * s - m) as the fp16 hi / lo A
+// operand.  The first block's alpha has two forms, equal in value but compiled differently: kScaleInPlace for attn_wide_kernel, which
+// scales O by alpha in place, and the other for the kernels that fold a per-block accumulator.  scale_log2e refers to the kernel
+// parameter, so it is read where it is used; held in a register across the block it costs attn_kernel one more register.
+template <bool kScaleInPlace>
+__device__ __forceinline__ void attn_softmax_step(const float (&S)[32], const int (&kv)[2], const float& scale_log2e, float (&m)[2],
+                                                  float (&l)[2], float (&alpha)[2], uint32_t (&Ph)[16], uint32_t (&Pl)[16]) {
+    const int lane = threadIdx.x & 31;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+        const int hr = (i >> 1) & 1;
+        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        if (col < kv[hr]) mx[hr] = fmaxf(mx[hr], S[i]);
+    }
+    float mn[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+        mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+        mn[hr] = fmaxf(m[hr], mx[hr] * scale_log2e);
+        if (kScaleInPlace)
+            alpha[hr] = m[hr] == -INFINITY ? 0.f : ex2_approx(m[hr] - mn[hr]);     // O and l are still zero before the first block
+        else    // a row that has seen no key yet keeps m = -inf: its weights are all zero (masked), nothing to rescale
+            alpha[hr] = mn[hr] == -INFINITY ? 1.f : ex2_approx(m[hr] - mn[hr]);
+    }
+    float ls[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+        const int hr = (i >> 1) & 1;
+        const int col = 8 * (i >> 2) + 2 * (lane & 3);
+        const float p0 = col < kv[hr] ? ex2_approx(fmaf(S[i], scale_log2e, -mn[hr])) : 0.f;
+        const float p1 = col + 1 < kv[hr] ? ex2_approx(fmaf(S[i + 1], scale_log2e, -mn[hr])) : 0.f;
+        ls[hr] += p0 + p1;
+        split_h16_pair(p0, p1, Ph[i >> 1], Pl[i >> 1]);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        l[hr] = l[hr] * alpha[hr] + ls[hr];
+        m[hr] = mn[hr];
+    }
+}
+
+// End of a query warpgroup: quad-reduces the row sums l, then stores O / l of query rows q0 and q0 + 8 (those below L) as fp16 planes:
+// NG groups of 8 columns from output column c0, of which those at or past ncols are skipped.  O[4 g + 2 hr], O[4 g + 2 hr + 1] are
+// columns 8 g + 2 (lane & 3), + 1 of row q0 + 8 hr.
+template <int NG>
+__device__ __forceinline__ void attn_store_rows(const AttnKernelParams& p, const float* O, float (&l)[2], int b, int q0, int c0,
+                                                int ncols) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 1);
+        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        const int grow = q0 + 8 * hr;
+        if (grow >= p.L) continue;
+        const float inv = 1.f / l[hr];
+        __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + c0 + 2 * (lane & 3);
+#pragma unroll
+        for (int g = 0; g < NG; ++g) {
+            const float v[2] = {O[4 * g + 2 * hr] * inv, O[4 * g + 2 * hr + 1] * inv};
+            if (8 * g < ncols) store_planes<2>(o, p.o_plane, 8 * g, v, 2);
         }
+    }
+}
+
+__global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_constant__ AttnKernelParams p) {
+    const AttnCta cta = attn_prologue<kAttnStages, kOffCtl, true>(p);
+    if (cta.wg == 0) {
+        if (threadIdx.x == 0) attn_produce(p, cta);
         return;
     }
 
     // ---------------------------------------------------------------------- query warpgroups
-    const int cw = wg - 1;
+    const int cw = cta.wg - 1;
     const int lane = threadIdx.x & 31;
     const int w = (threadIdx.x >> 5) & 3;
     const int r0 = cw * 64 + 16 * w + (lane >> 2);          // query rows r0 and r0 + 8 of the tile
-    const int q0 = qt * 128 + r0;
-    const uint32_t sq = smem_u32(smem) + cw * 64 * 128;
+    const int q0 = cta.qt * 128 + r0;
+    const uint32_t sq = smem_u32(cta.smem) + cw * 64 * 128;
     float O[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) O[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
-    mbar_wait(&ctl->q_full, 0);
-    for (int j = 0; j < nkv; ++j) {
+    mbar_wait(&cta.ctl->q_full, 0);
+    for (int j = 0; j < cta.nkv; ++j) {
         const int s = j % kAttnStages;
-        mbar_wait(&ctl->kv_full[s], (j / kAttnStages) & 1);
-        const uint32_t sk = smem_u32(smem + kOffKV + s * kStageBytes);
+        mbar_wait(&cta.ctl->kv_full[s], (j / kAttnStages) & 1);
+        const uint32_t sk = smem_u32(cta.smem + kOffKV + s * kStageBytes);
         const uint32_t sv = sk + kKBytes;
         float S[32];
         wgmma_fence();
@@ -137,46 +227,16 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
         wgmma_wait<0>();
         wgmma_fence_regs(S);
 
-        // S fragment: S[4 g + e] is row r0 + 8 (e >> 1), key j * 64 + 8 g + 2 (lane & 3) + (e & 1)
-        float mx[2] = {-INFINITY, -INFINITY};
         int kv[2];
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
             int lim = p.Lk - j * 64;
             if (p.causal) lim = min(lim, q0 + 8 * hr - j * 64 + 1);
-            kv[hr] = lim;                                     // keys of this block the row may see: column c valid iff c < kv
+            kv[hr] = lim;                                     // keys of this block the row may see
         }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-            const int hr = (i >> 1) & 1;
-            const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-            if (col < kv[hr]) mx[hr] = fmaxf(mx[hr], S[i]);
-        }
-        float alpha[2], mn[2];
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
-            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
-            mn[hr] = fmaxf(m[hr], mx[hr] * p.scale_log2e);
-            // a row that has seen no key yet keeps m = -inf: its weights are all zero (masked), nothing to rescale
-            alpha[hr] = mn[hr] == -INFINITY ? 1.f : ex2_approx(m[hr] - mn[hr]);
-        }
+        float alpha[2];
         uint32_t Ph[16], Pl[16];
-        float ls[2] = {0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-            const int hr = (i >> 1) & 1;
-            const int col = 8 * (i >> 2) + 2 * (lane & 3);
-            const float p0 = col < kv[hr] ? ex2_approx(fmaf(S[i], p.scale_log2e, -mn[hr])) : 0.f;
-            const float p1 = col + 1 < kv[hr] ? ex2_approx(fmaf(S[i + 1], p.scale_log2e, -mn[hr])) : 0.f;
-            ls[hr] += p0 + p1;
-            split_h16_pair(p0, p1, Ph[i >> 1], Pl[i >> 1]);
-        }
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-            l[hr] = l[hr] * alpha[hr] + ls[hr];
-            m[hr] = mn[hr];
-        }
+        attn_softmax_step<false>(S, kv, p.scale_log2e, m, l, alpha, Ph, Pl);
 
         // Ob = P V of this key block: k-chunk kc (keys 16 kc .. +15) of P is S registers 8 kc .. 8 kc + 7, i.e. Ph / Pl [4 kc .. 4 kc + 3];
         // the two correction passes (Pl V_hi, Ph V_lo) first.  The block's product gets its own accumulator and is folded into O below
@@ -199,28 +259,11 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(Ob);
-        if ((threadIdx.x & 127) == 0) mbar_arrive(&ctl->kv_empty[s]);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&cta.ctl->kv_empty[s]);
 #pragma unroll
         for (int i = 0; i < 32; ++i) O[i] = fmaf(O[i], alpha[(i >> 1) & 1], Ob[i]);
     }
-
-#pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 1);
-        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
-    }
-#pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-        const int grow = q0 + 8 * hr;
-        if (grow >= p.L) continue;
-        const float inv = 1.f / l[hr];
-        __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * 64 + 2 * (lane & 3);
-#pragma unroll
-        for (int g = 0; g < 8; ++g) {
-            const float v[2] = {O[4 * g + 2 * hr] * inv, O[4 * g + 2 * hr + 1] * inv};
-            store_planes<2>(o, p.o_plane, 8 * g, v, 2);
-        }
-    }
+    attn_store_rows<8>(p, O, l, cta.b, q0, cta.h * 64, 64);
 }
 
 // Heads of width 32, two per CTA (ds_attn_desc.pad0 == 32).  The loads are those of attn_kernel with a head PAIR in place of a
@@ -231,57 +274,18 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_kernel(const __grid_cons
 //   O_e = alpha_e O_e + P_e V_e   m64n32k16 with B at V^T rows 32 e .. 32 e + 31 (4096 B: whole 1024-byte swizzle atoms)
 // Against 64-wide zero-padded heads this halves the MMAs, the K / V^T bytes and the q/k/v/out GEMM widths.
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_pair_kernel(const __grid_constant__ AttnKernelParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    AttnCtl* ctl = reinterpret_cast<AttnCtl*>(smem + kOffCtl);
-
-    const int wg = threadIdx.x >> 7;
-    const int qt = blockIdx.x % p.q_tiles;
-    const int z = blockIdx.x / p.q_tiles;
-    const int hp = z % p.nh;                        // head pair
-    const int b = z / p.nh;
-    const int lk_eff = p.causal ? min(p.Lk, qt * 128 + 128) : p.Lk;
-    const int nkv = (lk_eff + 63) >> 6;
-
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&p.tmQ);
-        tma_prefetch_desc(&p.tmK);
-        tma_prefetch_desc(&p.tmV);
-        mbar_init(&ctl->q_full, 1);
-        for (int s = 0; s < kAttnStages; ++s) {
-            mbar_init(&ctl->kv_full[s], 1);
-            mbar_init(&ctl->kv_empty[s], 2);
-        }
-        fence_barrier_init();
-    }
-    __syncthreads();
-
-    if (wg == 0) {
-        if (threadIdx.x == 0) {
-            mbar_arrive_expect_tx(&ctl->q_full, kQBytes);
-            tma_load_3d(&p.tmQ, &ctl->q_full, smem, p.q_c0 + hp * 64, qt * 128, b);
-            tma_load_3d(&p.tmQ, &ctl->q_full, smem + 16384, p.q_c0 + hp * 64, qt * 128, p.B + b);
-            for (int j = 0; j < nkv; ++j) {
-                const int s = j % kAttnStages;
-                const uint32_t ph = (j / kAttnStages) & 1;
-                mbar_wait(&ctl->kv_empty[s], ph ^ 1);
-                mbar_arrive_expect_tx(&ctl->kv_full[s], kStageBytes);
-                uint8_t* sk = smem + kOffKV + s * kStageBytes;
-                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk, p.k_c0 + hp * 64, j * 64, b);
-                tma_load_3d(&p.tmK, &ctl->kv_full[s], sk + 8192, p.k_c0 + hp * 64, j * 64, p.B + b);
-                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes, j * 64, hp * 64, b);
-                tma_load_3d(&p.tmV, &ctl->kv_full[s], sk + kKBytes + 8192, j * 64, hp * 64, p.B + b);
-            }
-        }
+    const AttnCta cta = attn_prologue<kAttnStages, kOffCtl, true>(p);    // cta.h: the head pair
+    if (cta.wg == 0) {
+        if (threadIdx.x == 0) attn_produce(p, cta);
         return;
     }
 
-    const int cw = wg - 1;
+    const int cw = cta.wg - 1;
     const int lane = threadIdx.x & 31;
     const int w = (threadIdx.x >> 5) & 3;
     const int r0 = cw * 64 + 16 * w + (lane >> 2);
-    const int q0 = qt * 128 + r0;
-    const uint32_t sq = smem_u32(smem) + cw * 64 * 128;
+    const int q0 = cta.qt * 128 + r0;
+    const uint32_t sq = smem_u32(cta.smem) + cw * 64 * 128;
     float O[2][16];
 #pragma unroll
     for (int e = 0; e < 2; ++e)
@@ -289,11 +293,11 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_pair_kernel(const __grid
         for (int i = 0; i < 16; ++i) O[e][i] = 0.f;
     float m[2][2] = {{-INFINITY, -INFINITY}, {-INFINITY, -INFINITY}}, l[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 
-    mbar_wait(&ctl->q_full, 0);
-    for (int j = 0; j < nkv; ++j) {
+    mbar_wait(&cta.ctl->q_full, 0);
+    for (int j = 0; j < cta.nkv; ++j) {
         const int s = j % kAttnStages;
-        mbar_wait(&ctl->kv_full[s], (j / kAttnStages) & 1);
-        const uint32_t sk = smem_u32(smem + kOffKV + s * kStageBytes);
+        mbar_wait(&cta.ctl->kv_full[s], (j / kAttnStages) & 1);
+        const uint32_t sk = smem_u32(cta.smem + kOffKV + s * kStageBytes);
         const uint32_t sv = sk + kKBytes;
         int kv[2];
 #pragma unroll
@@ -321,37 +325,9 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_pair_kernel(const __grid
             wgmma_wait<0>();
             wgmma_fence_regs(S);
 
-            float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                const int hr = (i >> 1) & 1;
-                const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-                if (col < kv[hr]) mx[hr] = fmaxf(mx[hr], S[i]);
-            }
-            float alpha[2], mn[2];
-#pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-                mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
-                mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
-                mn[hr] = fmaxf(m[e][hr], mx[hr] * p.scale_log2e);
-                alpha[hr] = mn[hr] == -INFINITY ? 1.f : ex2_approx(m[e][hr] - mn[hr]);
-            }
+            float alpha[2];
             uint32_t Ph[16], Pl[16];
-            float ls[2] = {0.f, 0.f};
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-                const int hr = (i >> 1) & 1;
-                const int col = 8 * (i >> 2) + 2 * (lane & 3);
-                const float p0 = col < kv[hr] ? ex2_approx(fmaf(S[i], p.scale_log2e, -mn[hr])) : 0.f;
-                const float p1 = col + 1 < kv[hr] ? ex2_approx(fmaf(S[i + 1], p.scale_log2e, -mn[hr])) : 0.f;
-                ls[hr] += p0 + p1;
-                split_h16_pair(p0, p1, Ph[i >> 1], Pl[i >> 1]);
-            }
-#pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-                l[e][hr] = l[e][hr] * alpha[hr] + ls[hr];
-                m[e][hr] = mn[hr];
-            }
+            attn_softmax_step<false>(S, kv, p.scale_log2e, m[e], l[e], alpha, Ph, Pl);
             // per-block accumulator folded into O with fp32 FMAs, as in attn_kernel
             float Ob[16];
 #pragma unroll
@@ -370,29 +346,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_pair_kernel(const __grid
 #pragma unroll
             for (int i = 0; i < 16; ++i) O[e][i] = fmaf(O[e][i], alpha[(i >> 1) & 1], Ob[i]);
         }
-        if ((threadIdx.x & 127) == 0) mbar_arrive(&ctl->kv_empty[s]);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&cta.ctl->kv_empty[s]);
     }
-
 #pragma unroll
-    for (int e = 0; e < 2; ++e) {
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-            l[e][hr] += __shfl_xor_sync(0xffffffffu, l[e][hr], 1);
-            l[e][hr] += __shfl_xor_sync(0xffffffffu, l[e][hr], 2);
-        }
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-            const int grow = q0 + 8 * hr;
-            if (grow >= p.L) continue;
-            const float inv = 1.f / l[e][hr];
-            __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + hp * 64 + e * 32 + 2 * (lane & 3);
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                const float v[2] = {O[e][4 * g + 2 * hr] * inv, O[e][4 * g + 2 * hr + 1] * inv};
-                store_planes<2>(o, p.o_plane, 8 * g, v, 2);
-            }
-        }
-    }
+    for (int e = 0; e < 2; ++e) attn_store_rows<4>(p, O[e], l[e], cta.b, q0, cta.h * 64 + e * 32, 32);
 }
 
 // Heads of width hd = 72 .. 128, a multiple of 8 (ds_attn_desc.pad0 = hd; open_clip ViT-g-14: 16 heads of 88).  One head per CTA as
@@ -415,67 +372,44 @@ static constexpr size_t kWideSmem = kWideOffCtl + 256 + 1024;
 static_assert(kWideSmem <= 227 * 1024, "attn_wide_kernel shared memory");
 
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_wide_kernel(const __grid_constant__ AttnKernelParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    AttnCtl* ctl = reinterpret_cast<AttnCtl*>(smem + kWideOffCtl);
-
-    const int wg = threadIdx.x >> 7;
-    const int qt = blockIdx.x % p.q_tiles;
-    const int z = blockIdx.x / p.q_tiles;
-    const int h = z % p.nh;
-    const int b = z / p.nh;
-    const int nkv = (p.Lk + 63) >> 6;
-
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&p.tmQ);
-        tma_prefetch_desc(&p.tmK);
-        tma_prefetch_desc(&p.tmV);
-        mbar_init(&ctl->q_full, 1);
-        for (int s = 0; s < kWideStages; ++s) {
-            mbar_init(&ctl->kv_full[s], 1);
-            mbar_init(&ctl->kv_empty[s], 2);
-        }
-        fence_barrier_init();
-    }
-    __syncthreads();
-
-    if (wg == 0) {
+    const AttnCta cta = attn_prologue<kWideStages, kWideOffCtl, false>(p);
+    if (cta.wg == 0) {
         if (threadIdx.x == 0) {
-            mbar_arrive_expect_tx(&ctl->q_full, kWideQBytes);
+            mbar_arrive_expect_tx(&cta.ctl->q_full, kWideQBytes);
             for (int pl = 0; pl < 2; ++pl)
                 for (int cb = 0; cb < 2; ++cb)
-                    tma_load_4d(&p.tmQ, &ctl->q_full, smem + pl * 32768 + cb * 16384, cb * 64, h, qt * 128, pl * p.B + b);
-            for (int j = 0; j < nkv; ++j) {
+                    tma_load_4d(&p.tmQ, &cta.ctl->q_full, cta.smem + pl * 32768 + cb * 16384, cb * 64, cta.h, cta.qt * 128, pl * p.B + cta.b);
+            for (int j = 0; j < cta.nkv; ++j) {
                 const int s = j % kWideStages;
-                mbar_wait(&ctl->kv_empty[s], ((j / kWideStages) & 1) ^ 1);
-                mbar_arrive_expect_tx(&ctl->kv_full[s], kWideStageBytes);
-                uint8_t* sk = smem + kWideQBytes + s * kWideStageBytes;
+                mbar_wait(&cta.ctl->kv_empty[s], ((j / kWideStages) & 1) ^ 1);
+                mbar_arrive_expect_tx(&cta.ctl->kv_full[s], kWideStageBytes);
+                uint8_t* sk = cta.smem + kWideQBytes + s * kWideStageBytes;
                 for (int pl = 0; pl < 2; ++pl) {
                     for (int cb = 0; cb < 2; ++cb)
-                        tma_load_4d(&p.tmK, &ctl->kv_full[s], sk + pl * 16384 + cb * 8192, cb * 64, h, j * 64, pl * p.B + b);
-                    tma_load_4d(&p.tmV, &ctl->kv_full[s], sk + kWideKBytes + pl * 16384, j * 64, 0, h, pl * p.B + b);
+                        tma_load_4d(&p.tmK, &cta.ctl->kv_full[s], sk + pl * 16384 + cb * 8192, cb * 64, cta.h, j * 64, pl * p.B + cta.b);
+                    tma_load_4d(&p.tmV, &cta.ctl->kv_full[s], sk + kWideKBytes + pl * 16384, j * 64, 0, cta.h, pl * p.B + cta.b);
                 }
             }
         }
         return;
     }
 
-    const int cw = wg - 1;
+    const int cw = cta.wg - 1;
     const int lane = threadIdx.x & 31;
     const int w = (threadIdx.x >> 5) & 3;
     const int r0 = cw * 64 + 16 * w + (lane >> 2);
-    const int q0 = qt * 128 + r0;
-    const uint32_t sq = smem_u32(smem) + cw * 64 * 128;
+    const int q0 = cta.qt * 128 + r0;
+    const uint32_t sq = smem_u32(cta.smem) + cw * 64 * 128;
     float O[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) O[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
-    mbar_wait(&ctl->q_full, 0);
-    for (int j = 0; j < nkv; ++j) {
+    mbar_wait(&cta.ctl->q_full, 0);
+    for (int j = 0; j < cta.nkv; ++j) {
         const int s = j % kWideStages;
-        mbar_wait(&ctl->kv_full[s], (j / kWideStages) & 1);
-        const uint32_t sk = smem_u32(smem + kWideQBytes + s * kWideStageBytes);
+        mbar_wait(&cta.ctl->kv_full[s], (j / kWideStages) & 1);
+        const uint32_t sk = smem_u32(cta.smem + kWideQBytes + s * kWideStageBytes);
         const uint32_t sv = sk + kWideKBytes;
         // Q descriptors are rebuilt per block rather than hoisted out of the key loop: kept live, they would be spilled
         uint32_t sqj = sq;
@@ -497,37 +431,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_wide_kernel(const __grid
         wgmma_wait<0>();
         wgmma_fence_regs(S);
 
-        const int kv = p.Lk - j * 64;                   // keys of this block: column c valid iff c < kv
-        float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-            const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-            if (col < kv) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], S[i]);
-        }
-        float alpha[2], mn[2];
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
-            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
-            mn[hr] = fmaxf(m[hr], mx[hr] * p.scale_log2e);
-            alpha[hr] = m[hr] == -INFINITY ? 0.f : ex2_approx(m[hr] - mn[hr]);     // O and l are still zero before the first block
-        }
+        const int kv[2] = {p.Lk - j * 64, p.Lk - j * 64};      // keys of this block, the same for both row halves: no causal mask
+        float alpha[2];
         uint32_t Ph[16], Pl[16];
-        float ls[2] = {0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-            const int hr = (i >> 1) & 1;
-            const int col = 8 * (i >> 2) + 2 * (lane & 3);
-            const float p0 = col < kv ? ex2_approx(fmaf(S[i], p.scale_log2e, -mn[hr])) : 0.f;
-            const float p1 = col + 1 < kv ? ex2_approx(fmaf(S[i + 1], p.scale_log2e, -mn[hr])) : 0.f;
-            ls[hr] += p0 + p1;
-            split_h16_pair(p0, p1, Ph[i >> 1], Pl[i >> 1]);
-        }
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-            l[hr] = l[hr] * alpha[hr] + ls[hr];
-            m[hr] = mn[hr];
-        }
+        attn_softmax_step<true>(S, kv, p.scale_log2e, m, l, alpha, Ph, Pl);
 #pragma unroll
         for (int i = 0; i < 64; ++i) O[i] *= alpha[(i >> 1) & 1];
         // O += P V: the two correction passes (Pl V_hi, Ph V_lo) first; d-rows 64 c .. 64 c + 63 of V^T are 8 KB into the tile
@@ -545,28 +452,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_wide_kernel(const __grid
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(O);
-        if ((threadIdx.x & 127) == 0) mbar_arrive(&ctl->kv_empty[s]);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&cta.ctl->kv_empty[s]);
     }
-
-#pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 1);
-        l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
-    }
-#pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-        const int grow = q0 + 8 * hr;
-        if (grow >= p.L) continue;
-        const float inv = 1.f / l[hr];
-        __half* o = p.out + ((long long)b * p.L + grow) * p.o_pitch + h * p.hd + 2 * (lane & 3);
-#pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-            for (int g = 0; g < 8; ++g) {
-                const float v[2] = {O[32 * c + 4 * g + 2 * hr] * inv, O[32 * c + 4 * g + 2 * hr + 1] * inv};
-                if (64 * c + 8 * g < p.hd) store_planes<2>(o, p.o_plane, 64 * c + 8 * g, v, 2);   // hd % 8 == 0: whole 8-column groups
-            }
-    }
+    // O[32 c + 4 g ..] is group 8 c + g: columns 64 c + 8 g of the head; hd % 8 == 0, so the groups below hd are whole
+    attn_store_rows<16>(p, O, l, cta.b, q0, cta.h * p.hd, p.hd);
 }
 
 // ------------------------------------------------------------------------------------------ host

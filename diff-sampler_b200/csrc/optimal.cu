@@ -6,6 +6,7 @@
 // Every reduction is a fixed tree (warp shuffles, then the warp totals in warp order) and nothing uses atomics, so two calls on the
 // same input are bit-identical.
 #include "ops.h"
+#include "block.cuh"
 #include <cuda_fp16.h>
 #include <math.h>
 
@@ -15,27 +16,6 @@ static constexpr int kOptThreads = 512;
 static constexpr int kOptWarps = kOptThreads / 32;
 
 static int opt_ok() { return cudaGetLastError() == cudaSuccess ? 0 : -1; }
-
-struct SumOp {
-    template <class T> __device__ T operator()(T a, T b) const { return a + b; }
-};
-struct MaxOp {
-    template <class T> __device__ T operator()(T a, T b) const { return a > b ? a : b; }
-};
-
-// Block-wide reduction with a fixed order: butterfly within each warp, then every thread folds the warp totals 0, 1, ... itself.
-template <int NW, class T, class Op>
-__device__ __forceinline__ T block_reduce(T v, Op op, T* sh) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
-    __syncthreads();                                   // `sh` may still be read by the previous reduction
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-    __syncthreads();
-    T r = sh[0];
-#pragma unroll
-    for (int i = 1; i < NW; ++i) r = op(r, sh[i]);
-    return r;
-}
 
 // ||x - y||^2 by one warp: fp32 differences, squares and sums in fp64 (the squares of fp32 values are exact in fp64).
 __device__ __forceinline__ double warp_dist2(const float* __restrict__ x, const float* __restrict__ y, int D) {
@@ -115,19 +95,7 @@ __global__ void __launch_bounds__(kOptThreads) opt_softmax_kernel(ds_opt_softmax
         int total = 0;
         for (int base = 0; base < N; base += kOptThreads) {
             const int i = base + tid;
-            const bool f = i < N && (double)(u[i] * inv) >= thr;
-            const unsigned bal = __ballot_sync(0xffffffffu, f);
-            __syncthreads();
-            if (lane == 0) shi[w] = __popc(bal);
-            __syncthreads();
-            int before = total, tile = 0;
-            for (int ww = 0; ww < kOptWarps; ++ww) {
-                if (ww < w) before += shi[ww];
-                tile += shi[ww];
-            }
-            before += __popc(bal & ((1u << lane) - 1u));
-            if (f && before < DS_OPT_CAP) band[before] = i;
-            total += tile;
+            total = block_compact<kOptWarps, DS_OPT_CAP>(i < N && (double)(u[i] * inv) >= thr, i, band, total, shi);
             if (total > DS_OPT_CAP) break;                 // block-uniform
         }
         __syncthreads();
@@ -174,22 +142,6 @@ __global__ void __launch_bounds__(256) opt_reduce_kernel(ds_opt_reduce_desc d) {
     }
 }
 
-// Block argmax over u (ties to the lower index); the winner is returned to every thread.
-__device__ __forceinline__ void block_argmax(float& v, int& idx, float* shf, int* shi) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float v2 = __shfl_xor_sync(0xffffffffu, v, o);
-        const int i2 = __shfl_xor_sync(0xffffffffu, idx, o);
-        if (v2 > v || (v2 == v && i2 < idx)) { v = v2; idx = i2; }
-    }
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) { shf[threadIdx.x >> 5] = v; shi[threadIdx.x >> 5] = idx; }
-    __syncthreads();
-    v = shf[0]; idx = shi[0];
-    for (int i = 1; i < kOptWarps; ++i)
-        if (shf[i] > v || (shf[i] == v && shi[i] < idx)) { v = shf[i]; idx = shi[i]; }
-}
-
 __global__ void __launch_bounds__(kOptThreads) opt_knn_kernel(ds_opt_knn_desc d) {
     __shared__ float shf[kOptWarps];
     __shared__ int shi[kOptWarps];
@@ -209,7 +161,7 @@ __global__ void __launch_bounds__(kOptThreads) opt_knn_kernel(ds_opt_knn_desc d)
             const float t = u[i];
             if (t > v || (t == v && i < idx)) { v = t; idx = i; }
         }
-        block_argmax(v, idx, shf, shi);
+        block_argbest<kOptWarps, true>(v, idx, shf, shi);
         if (idx == 0x7fffffff) break;
         if (cnt >= d.k && (double)v < kth - 2.0 * err) break;
         if (tid == 0) { cand[cnt] = idx; u[idx] = -INFINITY; }

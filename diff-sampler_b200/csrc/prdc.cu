@@ -9,6 +9,7 @@
 // Counts are integer sums and the realism a maximum, the ranks of the radius candidates are total orders, and nothing uses atomics: two
 // calls on the same input are bit-identical.
 #include "ops.h"
+#include "block.cuh"
 #include <math.h>
 
 namespace dsb {
@@ -55,62 +56,11 @@ __device__ __forceinline__ double warp_exact_d2(const double* __restrict__ x, co
     return s;
 }
 
-template <class T>
-__device__ __forceinline__ T block_sum(T v, T* sh) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-    __syncthreads();
-    T r = sh[0];
-    for (int i = 1; i < kPrdcWarps; ++i) r += sh[i];
-    return r;
-}
-
-__device__ __forceinline__ double block_max(double v, double* sh) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double r = sh[0];
-    for (int i = 1; i < kPrdcWarps; ++i) r = fmax(r, sh[i]);
-    return r;
-}
-
-// Block argmin (ties to the lower index); the winner is returned to every thread.
-__device__ __forceinline__ void block_argmin(float& v, int& idx, float* shf, int* shi) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float v2 = __shfl_xor_sync(0xffffffffu, v, o);
-        const int i2 = __shfl_xor_sync(0xffffffffu, idx, o);
-        if (v2 < v || (v2 == v && i2 < idx)) { v = v2; idx = i2; }
-    }
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) { shf[threadIdx.x >> 5] = v; shi[threadIdx.x >> 5] = idx; }
-    __syncthreads();
-    v = shf[0]; idx = shi[0];
-    for (int i = 1; i < kPrdcWarps; ++i)
-        if (shf[i] < v || (shf[i] == v && shi[i] < idx)) { v = shf[i]; idx = shi[i]; }
-}
-
-// Appends index i of every flagged thread of one kPrdcThreads-wide tile to list[n ..] in index order (warp ballots); returns the new
-// length, the same in every thread.  The caller synchronises before reading the list.
-__device__ __forceinline__ int append_tile(bool f, int i, int* list, int n, int* shi) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const unsigned bal = __ballot_sync(0xffffffffu, f);
-    __syncthreads();
-    if (lane == 0) shi[w] = __popc(bal);
-    __syncthreads();
-    int before = n, tile = 0;
-    for (int ww = 0; ww < kPrdcWarps; ++ww) {
-        if (ww < w) before += shi[ww];
-        tile += shi[ww];
-    }
-    before += __popc(bal & ((1u << lane) - 1u));
-    if (f) list[before] = i;
-    return n + tile;
-}
+// The realism maximum takes fmax, not MaxOp: fmax drops a nan operand wherever it stands, so the maximum covers the ratios that are
+// numbers whatever the order; a nan ratio is counted in nan_seen and wins there, as in numpy.
+struct FmaxOp {
+    __device__ double operator()(double a, double b) const { return fmax(a, b); }
+};
 
 // The list is flushed once it holds more than this, so one more tile always fits.
 static constexpr int kFlushAt = DS_PRDC_LIST - kPrdcThreads;
@@ -140,7 +90,7 @@ __global__ void __launch_bounds__(kPrdcThreads) prdc_kth_kernel(ds_prdc_kth_desc
             const float t = a[i];
             if (t < v || (t == v && i < idx)) { v = t; idx = i; }
         }
-        block_argmin(v, idx, shf, shi);
+        block_argbest<kPrdcWarps, false>(v, idx, shf, shi);
         hi = fmax(hi, (double)v + d2_bound(qn2, d.tn2[idx], d.sq, d.st, D));
         if (tid == 0) { bidx[c] = idx; a[idx] = INFINITY; }
         __syncthreads();
@@ -152,7 +102,7 @@ __global__ void __launch_bounds__(kPrdcThreads) prdc_kth_kernel(ds_prdc_kth_desc
     int n = 0, rescored = kk;
     for (int base = 0; base < N; base += kPrdcThreads) {
         const int i = base + tid;
-        n = append_tile(i < N && (double)a[i] - d2_bound(qn2, d.tn2[i], d.sq, d.st, D) <= hi, i, list, n, shi);
+        n = block_compact<kPrdcWarps>(i < N && (double)a[i] - d2_bound(qn2, d.tn2[i], d.sq, d.st, D) <= hi, i, list, n, shi);
         const bool last = base + kPrdcThreads >= N;
         if (n <= kFlushAt && !last) continue;                 // block-uniform
         __syncthreads();
@@ -216,7 +166,7 @@ __global__ void __launch_bounds__(kPrdcThreads) prdc_count_kernel(ds_prdc_count_
             if (real && d.tau[i] < d.med && a + B > 0.0)
                 lo_best = fmax(lo_best, d.tau[i] / sqrt(a + B) * (1.0 - 0x1p-40));
         }
-        n = append_tile(und, i, list, n, shi);
+        n = block_compact<kPrdcWarps>(und, i, list, n, shi);
         if (n <= kFlushAt && base + kPrdcThreads < N) continue;
         __syncthreads();
         for (int j = w; j < n; j += kPrdcWarps) {
@@ -231,11 +181,11 @@ __global__ void __launch_bounds__(kPrdcThreads) prdc_count_kernel(ds_prdc_count_
         __syncthreads();
         n = 0;
     }
-    ct = block_sum(ct, shi);
-    co = block_sum(co, shi);
+    ct = block_reduce<kPrdcWarps>(ct, SumOp(), shi);
+    co = block_reduce<kPrdcWarps>(co, SumOp(), shi);
     if (real) {
         // every masked pair whose ratio could reach the best lower bound is recomputed; the others cannot hold the maximum
-        lo_best = block_max(lo_best, shd);
+        lo_best = block_reduce<kPrdcWarps>(lo_best, FmaxOp(), shd);
         double best = -INFINITY;
         int nan_seen = 0;
         for (int base = 0; base < N; base += kPrdcThreads) {
@@ -247,7 +197,7 @@ __global__ void __launch_bounds__(kPrdcThreads) prdc_count_kernel(ds_prdc_count_
                 const double lo = a - d2_bound(qn2, tn2, d.sq, d.st, D);
                 cand = !(lo > 0.0) || d.tau[i] / sqrt(lo) * (1.0 + 0x1p-40) >= lo_best;
             }
-            n = append_tile(cand, i, list, n, shi);
+            n = block_compact<kPrdcWarps>(cand, i, list, n, shi);
             if (n <= kFlushAt && base + kPrdcThreads < N) continue;
             __syncthreads();
             for (int j = w; j < n; j += kPrdcWarps) {
@@ -262,11 +212,11 @@ __global__ void __launch_bounds__(kPrdcThreads) prdc_count_kernel(ds_prdc_count_
             __syncthreads();
             n = 0;
         }
-        best = block_max(best, shd);
-        nan_seen = block_sum(nan_seen, shi);
+        best = block_reduce<kPrdcWarps>(best, FmaxOp(), shd);
+        nan_seen = block_reduce<kPrdcWarps>(nan_seen, SumOp(), shi);
         if (tid == 0) d.realism[b] = nan_seen ? NAN : best;
     }
-    rescored = block_sum(rescored, shi);
+    rescored = block_reduce<kPrdcWarps>(rescored, SumOp(), shi);
     if (tid == 0) {
         d.cnt_t[b] = ct;
         if (own) d.cnt_own[b] = co;
